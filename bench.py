@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — images/sec of the LSeg forward path (480x480, ADE20K-150) on 1..8 B200.
+"""bench.py — images/sec of the LSeg forward path (480x480, ADE20K-150) on 1..8 H100.
 
 One "step" = one LSegNet.forward over one batch of synthetic images (BASELINE.json configs[1]: batch 8 per GPU, K=150,
 480x480, ViT-L/16 DPT); at N > 1 the step is BASELINE.json configs[2]: the batch shards over the ranks and the logits of
-all shards are gathered on rank 0 INSIDE the timed region (lang-seg_b200/parallel.py::LogitsGather). Contract: see the
-task prompt / DESIGN.md section "Measurement". Prints ONE JSON line on rank 0.
+all shards are gathered on rank 0 INSIDE the timed region (lang-seg_b200/parallel.py::LogitsGather). Per-step time is
+CUDA events around each step with the L2 flushed (untimed) in between; prints ONE JSON line on rank 0.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # B200 arm
+  python bench.py [--gpus N] [--steps K] [--warmup W]            # GPU arm
+  python bench.py --dump-outputs DIR                             # + the last timed step's logits (seeded sample) as .npy
   python bench.py --impl reference [--steps K] [--warmup W]      # the reference's own CPU path on the host cores
   python bench.py --config 5                                     # BASELINE.json configs[4]: 736^2 (720 padded), K=512, B=4/GPU
 """
@@ -38,12 +39,14 @@ def ade_labels():
 
 
 def measured_peaks():
+    """(sustained, burst) dense fp16 tensor TFLOP/s and HBM GB/s used as roofline denominators: MEASURED_PEAKS.json when
+    present, else NVIDIA's H100 SXM data sheet (989 TFLOP/s dense fp16, 3350 GB/s) — a bound, not a reached rate."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return (p.get("bf16_tflops_sustained", 1428.7), p.get("bf16_tflops", 1692.4), p.get("hbm_gbs", 6564.2), "measured")
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return (p.get("bf16_tflops_sustained", 989.0), p.get("bf16_tflops", 989.0), p.get("hbm_gbs", 3350.0), "measured")
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -126,39 +129,23 @@ def _calibrate_threads(fn):
 
 
 def cpu_reference_rate(steps, warmup, labels, size):
-    """images/sec of the reference's CPU path, one image of the workload per step.
-
-    kind "reference": the UNMODIFIED reference `LSegModule.evaluate_random` (modules/lsegmentation_module.py:54-59 ->
-    modules/models/lseg_net.py:160-205) from baseline/_ref (oracle/make_ref.sh), with the stand-ins of
-    oracle/ref_standins.py for the absent third-party packages; kind "port": the oracle restatement when the reference
-    tree is not installed. The reference re-runs the text tower on every call (lseg_net.py:183); `text_cached` subtracts
-    a separately timed encode_text so that both accountings are visible."""
-    from oracle import ref_standins as R
+    """images/sec of the reference's CPU path, one image of the workload per step, through the oracle's restatement of
+    it (oracle/lseg_oracle.py, pinned to the reference by the golden fixtures). The reference re-runs the text tower on
+    every call (lseg_net.py:183); `text_cached` subtracts a separately timed encode_text so that both accountings are
+    visible."""
+    from oracle import lseg_oracle as O
     from oracle import synth
     sd = synth.make_state_dict(0)
     x_small = synth.make_image(1, 160, 160, seed=0)
     x = synth.make_image(1, size, size, seed=0)
-    if R.reference_available():
-        module = R.build_reference_module(sd, drop_in=False)
-        kind = "reference"
+    tw = O.clip_text_weights_fp16(sd)
+    kind = "port"
 
-        def fwd(img, lab):
-            with torch.no_grad():
-                return module.evaluate_random(img, lab)
+    def fwd(img, lab):
+        return O.lseg_forward(img, synth.tokenize(lab), sd, tw)
 
-        def text_only(lab):
-            with torch.no_grad():
-                return module.net.clip_pretrained.encode_text(synth.tokenize(lab))
-    else:
-        from oracle import lseg_oracle as O
-        tw = O.clip_text_weights_fp16(sd)
-        kind = "port"
-
-        def fwd(img, lab):
-            return O.lseg_forward(img, synth.tokenize(lab), sd, tw)
-
-        def text_only(lab):
-            return O.clip_encode_text(synth.tokenize(lab), tw)
+    def text_only(lab):
+        return O.clip_encode_text(synth.tokenize(lab), tw)
     cores = _calibrate_threads(lambda: fwd(x_small, labels[:8]))
     for _ in range(warmup):
         fwd(x, labels)
@@ -199,16 +186,32 @@ def line_config(cfg, args, world):
     """The `config` object of the JSON line — the SAME dict in both arms (`--impl b200` and `--impl reference` describe one
     workload; what differs between the arms is said per arm inside the values, and the reference arm's bounded sample is
     in its `cpu_baseline.sample`)."""
-    par = f"B200 arm: dp{world}, batch shard per rank, no collective on the image path"
+    par = f"GPU arm: dp{world}, batch shard per rank, no collective on the image path"
     if world > 1:
         par += f"; all shards' logits gathered on rank 0 inside the timed step ({args.gather})"
     par += "; reference arm: the host cores of rank 0"
     return dict(cfg["config"], backbone=args.backbone, global_batch=cfg["batch"] * world, parallelism=par,
                 weights="random init of the architecture",
-                text_features="B200 arm: cached per label set; reference arm: re-run on every call as the reference does "
+                text_features="GPU arm: cached per label set; reference arm: re-run on every call as the reference does "
                               "(cpu_baseline.value_text_cached = the same run with the text tower subtracted)",
-                l2="B200 arm, N=1: 256 MiB flush (untimed) between timed steps; N>1: back-to-back steps, per-step working "
-                   "set ~3.7 GB >> 126 MB L2")
+                l2="GPU arm, N=1: 256 MiB flush (untimed) between timed steps; N>1: back-to-back steps, per-step working "
+                   "set ~3.7 GB >> 50 MB L2")
+
+
+def dump_outputs(path, out):
+    """The logits [B, K, S, S] of the last timed step, reduced to at most 56 MB: every s-th pixel of every row and column
+    (s = 8, or the smallest larger stride that keeps the lattice within 48 MB), and 2M positions drawn from a fixed seed
+    (the same positions for the same shape in every run)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    B, K, H, W = out.shape
+    s = 8
+    while B * K * (-(-H // s)) * (-(-W // s)) * 4 > (48 << 20):
+        s += 1
+    np.save(os.path.join(path, "logits_lattice.npy"), out[:, :, ::s, ::s].float().cpu().numpy())
+    g = torch.Generator(device="cpu").manual_seed(0)
+    idx = torch.randint(0, out.numel(), (min(out.numel(), 1 << 21),), generator=g)
+    np.save(os.path.join(path, "logits_sample.npy"), out.reshape(-1)[idx.to(out.device)].float().cpu().numpy())
 
 
 def make_config(args):
@@ -257,6 +260,10 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-eval", action="store_true", help="skip the multi-scale evaluator line (SURVEY 8(f) row 1)")
     ap.add_argument("--dump-profile", default=None, help="write the per-launch profile of one step to this JSON file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float32): the logits on a regular "
+                         "pixel lattice (stride 8, coarser for outputs too large for 48 MB) and at a fixed seeded sample "
+                         "of 2M positions")
     args = ap.parse_args()
     cfg = make_config(args)
     if args.impl == "reference":
@@ -266,7 +273,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     numa = bind_to_gpu_numa(local_rank)
@@ -294,7 +301,7 @@ def main():
     x = x_host.to(dev)
     eng = net._engine_for(dev)
     text = net._text_features(eng, tokens)  # encoded once, cached (steady state of a fixed label set)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -331,12 +338,14 @@ def main():
     t_wall = time.perf_counter() - t_wall0
     clocks = sampler.summary() if world == 1 else None
     compute_ms = max_over_ranks(sum(s.elapsed_time(e) for s, e in zip(starts, ends)))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     compute_value = world * B * Ksteps / (compute_ms / 1e3)
 
     # ---- N > 1: the step of BASELINE.json configs[2] — forward + gather of all shards' logits on rank 0, timed as a whole.
     # The steps run back to back (the gather of step i overlaps the compute of step i+1 on a side stream), one event pair
     # around all K steps including the drain of the last gather; no flush kernel in between: a step streams ~3 GB of
-    # activations and 0.7 GB of weights through the 126 MB L2, nothing of step i survives into step i+1.
+    # activations and 0.7 GB of weights through the 50 MB L2, nothing of step i survives into step i+1.
     gather_info = None
     value, total_ms = compute_value, compute_ms
     if dist is not None:
@@ -369,7 +378,16 @@ def main():
 
         # Load-balanced variant: rank 0 also expands every shard to fp32 (t_up per image, serialised with its trunk), so it
         # computes fewer images itself: the largest root batch whose step fits the other ranks' (which skip the expansion).
-        t_up = 0.0285 * (K * S * S) / (150.0 * 480 * 480)             # ms per image, measured (profiles/r02_upsample*)
+        lr = eng.forward_lowres(x, text, K)
+        ops.upsample2x_nchw(lr)
+        u0, u1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        u0.record()
+        for _ in range(5):
+            ops.upsample2x_nchw(lr)
+        u1.record()
+        torch.cuda.synchronize()
+        t_up = max_over_ranks(u0.elapsed_time(u1) / (5 * B))             # ms per image of the fp32 expansion, measured
+        del lr
         t_img = max(1e-3, compute_ms / Ksteps / B - t_up)              # ms per image of the trunk
         root_batch = B
         while root_batch > 1 and root_batch * t_img + (root_batch + (world - 1) * B) * t_up > B * t_img:
@@ -420,7 +438,7 @@ def main():
         g.close()
         out = torch.empty((B, K, S, S), dtype=torch.float32, device=dev)
 
-    # ---- roofline of the dominant kernel family (tcgen05 GEMM) + MHSA: per-launch CUDA events, one step ----
+    # ---- roofline of the dominant kernel family (wgmma GEMM) + MHSA: per-launch CUDA events, one step ----
     peak_tf, peak_burst, peak_gbs, peak_src = measured_peaks()
     roofline, mhsa_roof, breakdown = None, None, None
     if rank == 0:
@@ -438,27 +456,17 @@ def main():
         g_ms_, g_fl, g_n = by[1]
         m_ms, m_fl, m_n = by[2]
         ach = g_fl / (g_ms_ / 1e3) / 1e12 if g_ms_ > 0 else 0.0
-        traffic, traffic_m = None, None  # DRAM bytes per launch from this round's committed ncu capture, if present
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-                tj = json.load(f)
-            traffic, traffic_m = tj["gemm"]["dram_bytes_per_launch"], tj["mhsa"]["dram_bytes_per_launch"]
-        except (OSError, KeyError, ValueError):
-            pass
-        roofline = {"kernel": "gemm_tc2_kernel (tcgen05 GEMM / implicit conv, all launches of one step)",
+        roofline = {"kernel": "gemm_tc_kernel (wgmma GEMM / implicit conv, all launches of one step)",
                     "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
                     "frac_of_burst_peak": ach / peak_burst,
-                    "peak_source": f"{peak_src} bf16 sustained (kernel timed inside a long step); burst peak {peak_burst}",
+                    "peak_source": f"{peak_src}: sustained {peak_tf}, burst {peak_burst}",
                     "launches": g_n, "avg_launch_ms": g_ms_ / max(g_n, 1), "share_of_step": g_ms_ / tot,
-                    "traffic": traffic,
-                    "traffic_note": "dram__bytes_read+write per launch (mean over the family) from the ncu capture "
-                                    "profiles/r02_traffic.md; per-shape table in profiles/r02_gemm_shapes.md",
                     "timing_note": "per-launch events serialise the programmatic-dependent-launch overlap of consecutive "
                                    "kernels: the breakdown sums to more than ms_per_step"}
         ach_m = m_fl / (m_ms / 1e3) / 1e12 if m_ms > 0 else 0.0
-        mhsa_roof = {"kernel": "mhsa2_kernel (lseg_mhsa_variant %s)" % os.environ.get("LSEG_MHSA_VARIANT", "0"),
+        mhsa_roof = {"kernel": "mhsa_kernel (lseg_mhsa_variant %s)" % os.environ.get("LSEG_MHSA_VARIANT", "0"),
                      "bound": "tensor", "achieved": ach_m, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach_m / peak_tf,
-                     "frac_of_burst_peak": ach_m / peak_burst, "launches": m_n, "traffic": traffic_m,
+                     "frac_of_burst_peak": ach_m / peak_burst, "launches": m_n,
                      "avg_launch_ms": m_ms / max(m_n, 1), "share_of_step": m_ms / tot}
         breakdown = {"gemm_ms": g_ms_, "mhsa_ms": m_ms, "layernorm_ms": by[3][0], "elementwise_ms": by[0][0],
                      "sum_ms": tot}

@@ -1,4 +1,4 @@
-/* lseg_b200 — C ABI of the B200-native LSeg forward path (liblseg_b200.so).
+/* lseg_b200 — C ABI of the H100-native LSeg forward path (liblseg_b200.so).
  *
  * Drop-in boundary for the hot path of isl-org/lang-seg: LSegNet.forward
  * (modules/models/lseg_net.py:160-205) and its zero-shot twin (modules/models/lseg_net_zs.py:177-214).
@@ -39,7 +39,7 @@ enum { LSEG_ACT_NONE = 0, LSEG_ACT_GELU = 1, LSEG_ACT_QUICKGELU = 2, LSEG_ACT_RE
 /* output addressing of the GEMM epilogue */
 enum { LSEG_STORE_ROWMAJOR = 0, LSEG_STORE_D2S = 1, LSEG_STORE_NCHW_T = 2 };
 
-/* One dense contraction  C[M,N] = epi(A[M,K] * W[N,K]^T)  on tcgen05 (k1,k4,k6-k8,k10-k17,k19).
+/* One dense contraction  C[M,N] = epi(A[M,K] * W[N,K]^T)  on wgmma (k1,k4,k6-k8,k10-k17,k19).
  * Replaces the torch Linear / Conv2d(1x1, 3x3 s1 p1) / ConvTranspose2d(k==s) calls listed in
  * SURVEY.md section 8(a): timm Block linears (lseg_vit.py:196-197), ProjectReadout (lseg_vit.py:79-90),
  * act_postprocess convs (lseg_vit.py:450-522), scratch.layerN_rn (lseg_blocks.py:73-108),
@@ -87,27 +87,24 @@ int lseg_gemm(const lseg_gemm_args* args, void* stream);
 /* Fused MHSA, head_dim 64 (k5; timm Attention restated at lseg_vit.py:26-39; CLIP text MHA).
  * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64]. */
 int lseg_mhsa(const void* qkv, void* out, int B, int N, int heads, int causal, void* stream);
-/* Same contract as lseg_mhsa with an explicit kernel choice (A/B measurements, tools/op_bench.py; the engine runs
- * variant 0 unless LSEG_MHSA_VARIANT overrides it — round 2 measured 1..8 within +-3 % of it, profiles/r02_mhsa_analysis.md): 0 = round-1 kernel (one polling MMA warp for both softmax streams);
- * 1 = one blocking MMA warp per stream + per-role register budgets (setmaxnreg); 2 = 1 + packed-fp32 (FFMA2 / FADD2 /
- * FMNMX3) softmax arithmetic; 3 = 2 + one of every four score pairs exponentiated on the FMA pipe; 4 = two of four;
- * 5..8 = the probabilities stay in tensor memory (tcgen05.st over the S tile, PV MMA with its A operand from TMEM):
- * 5 scalar softmax arithmetic, 6 packed, 7 packed + one of four pairs on the FMA pipe, 8 two of four. */
+/* Same contract as lseg_mhsa with an explicit kernel choice (A/B measurements; the engine runs variant 0 unless
+ * LSEG_MHSA_VARIANT overrides it). One wgmma flash-attention kernel; the variants differ in how many exponentials are
+ * evaluated on the FMA pipe instead of the MUFU pipe: 0, 1, 2, 5, 6 = none; 3, 7 = one of every four score pairs;
+ * 4, 8 = two of four. */
 int lseg_mhsa_variant(const void* qkv, void* out, int B, int N, int heads, int causal, int variant, void* stream);
 /* Causal attention of the CLIP text tower with the rounding points of torch's multi_head_attention_forward on fp16
  * tensors (q*dh^-0.5, bmm -> fp16, softmax -> fp16 normalised, bmm -> fp16; SURVEY.md Appendix A.2): CUDA cores, one
  * CTA per (label, head). qkv fp16 [K, L, 3*heads*64] -> out fp16 [K*L, heads*64], L <= 80. */
 int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* stream);
 /* 1 (default): every floating-point sum is formed in a fixed order (bit-reproducible across runs and batch sizes).
- * 0 (or LSEG_SPLITK=1): the in-place residual GEMM of the MLP (fc2) may split a tile's K range over two CTA pairs whose
- * partial sums are reduce-added in arrival order (differences at the fp32 rounding level; fc2 55 -> 51 us in
- * isolation, not visible in the end-to-end step time, hence off). */
+ * 0 (or LSEG_SPLITK=1): the in-place residual GEMM of the MLP (fc2) may split a tile's K range over two CTAs whose
+ * partial sums are reduce-added in arrival order (differences at the fp32 rounding level, hence off by default). */
 int lseg_set_deterministic(int on);
-/* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTA pairs
+/* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTAs
  * into trace ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). */
 int lseg_debug_gemm_trace(unsigned long long* trace);
 /* Debug: same computation, additionally stamps clock64() at the pipeline hand-off points of 16 sampled CTAs into
- * trace ([16][10 warps][256] uint64 device memory, zero-initialised by the caller); tools/mhsa_trace.py. */
+ * trace ([16][10 warps][256] uint64 device memory, zero-initialised by the caller). */
 int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int causal, unsigned long long* trace,
                     void* stream);
 
@@ -341,7 +338,7 @@ int lseg_forward_argmax(lseg_engine* e, const float* x, int B, int H, int W, con
                         long long text_image_stride, long long* mask, float* logits, void* stream);
 
 /* Same as lseg_forward, but brackets every kernel launch with CUDA events on `stream`, synchronises,
- * and returns per-launch device time (ms), kernel class (0 elementwise, 1 tcgen05 GEMM, 2 MHSA,
+ * and returns per-launch device time (ms), kernel class (0 elementwise, 1 wgmma GEMM, 2 MHSA,
  * 3 LayerNorm) and ALGORITHMIC flops of the launch. Used by bench.py for the roofline block. */
 int lseg_forward_profiled(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
                           long long text_image_stride, float* out, void* stream, float* step_ms, int* step_kind,

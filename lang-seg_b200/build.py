@@ -1,4 +1,4 @@
-"""Build liblseg_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build liblseg_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
 The library is a single translation unit (csrc/lseg_b200.cu) linked against the static CUDA runtime
 only; the driver API entry point it needs (cuTensorMapEncodeTiled) is resolved at run time, so the
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblseg_b200.so")
 SOURCES = ["lseg_b200.cu"]
-HEADERS = ["common.cuh", "gemm_tc.cuh", "mhsa.cuh", "mhsa2.cuh", "mhsa3.cuh", "mhsa4.cuh", "text_attn.cuh", "p2p.cuh", "evaluator.cuh", "elementwise.cuh", "engine.cuh"]
+HEADERS = ["common.cuh", "gemm_tc.cuh", "mhsa.cuh", "text_attn.cuh", "p2p.cuh", "evaluator.cuh", "elementwise.cuh", "engine.cuh"]
 
 
 def nvcc_path():
@@ -48,7 +48,7 @@ def build(force=False, verbose=False):
             tmp = f"{LIB}.tmp{os.getpid()}"
             cmd = [
                 nvcc_path(),
-                "-gencode", "arch=compute_100a,code=sm_100a",
+                "-gencode", "arch=compute_90a,code=sm_90a",
                 "-O3", "-std=c++17", "-lineinfo",
                 "-shared", "-Xcompiler", "-fPIC",
                 "-cudart", "static",

@@ -1,8 +1,7 @@
-// lseg_b200 — shared device helpers for the sm_100a kernels.
+// lseg_b200 — shared device helpers for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers (mbarrier, TMA, tcgen05/TMEM), UMMA descriptor builders and the
-// host-side tensor-map factory. Everything here is written for sm_100a only; there is no
-// fallback path.
+// Thin inline-PTX wrappers (mbarrier, TMA, wgmma), shared-memory matrix descriptors and the host-side
+// tensor-map factory. Everything here is written for sm_90a (Hopper) only; there is no fallback path.
 #pragma once
 #include <cstdlib>
 #include <cuda.h>
@@ -41,7 +40,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 // suspend-time hint: the waiting thread sleeps in hardware until the phase completes or this many ns
 // pass, instead of re-polling every ~100 cycles and stealing issue slots from the compute warps that
-// share its SM sub-partition (ncu: 3.1 M TRYWAIT re-issues per MHSA launch without the hint).
+// share its SM sub-partition.
 constexpr uint32_t kTryWaitHintNs = 20000;
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -152,16 +151,16 @@ __device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity, i
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------
 // Every per-step kernel is launched with programmaticStreamSerializationAllowed: its CTAs may become resident and
-// run their prologue (barrier init, TMEM alloc, tensor-map prefetch) while the previous kernel of the stream is
+// run their prologue (barrier init, tensor-map prefetch) while the previous kernel of the stream is
 // still draining. griddep_wait() blocks until that previous grid has completed and its writes are visible; it
 // must precede the first access to any global memory another kernel of the step reads or writes.
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // One lane of a converged warp (elect.sync): the MMA / TMA warps run converged with warp-uniform values (which the
-// compiler then keeps in uniform registers) and only predicate the tcgen05 / bulk-copy instruction itself on this
+// compiler then keeps in uniform registers) and only predicate the bulk-copy instruction itself on this
 // — a `if (lane == 0) { ... }` region makes every descriptor operand go through an ELECT + R2UR waterfall
-// (~20 dependent instructions, ~130 clk per tcgen05.mma measured).
+// (~20 dependent instructions per issue).
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -173,13 +172,12 @@ __device__ __forceinline__ bool elect_one_sync() {
 }
 __device__ __forceinline__ int warp_idx_sync() { return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0); }
 
+
 // ---- proxies / fences --------------------------------------------------------------------
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---- TMA ---------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -234,185 +232,66 @@ __device__ __forceinline__ void tma_store_wait_read() {
 
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- TMEM --------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns; thread t of the warp receives lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM, same 32 lanes x 32 columns shape as tmem_ld32
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-// 8- and 16-column variants (keep register pressure low on rarely taken paths)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- UMMA (tcgen05.mma) ------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type 2 at bits [61,64), descriptor
-// version 1 at bits [46,48)). Addresses / offsets are encoded >>4. Tiles must be 1024 B aligned.
-//   K-major operand (rows of 64 halves = 128 B): SBO = 1024 B between 8-row groups, LBO unused.
-//   MN-major operand (128 B along MN per K index): SBO = 1024 B between 8-k groups,
-//   LBO = byte stride between 64-element MN chunks.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
+// ---- wgmma (warpgroup MMA) -----------------------------------------------------------------
+// Shared-memory matrix descriptor, 128-byte swizzle (layout type 1 at bits [62,64)); addresses / offsets are encoded
+// >>4. Tiles are 1024 B aligned (the 8-row swizzle atom), so the base-offset field stays 0.
+//   K-major operand (rows of 64 halves = 128 B, as TMA writes a {64, rows} box): SBO = 1024 B between 8-row groups,
+//   LBO unused; the k-th 16-element K slice starts k * 32 B into the tile.
+//   MN-major operand (128 B along MN per K index, i.e. a row-major [K, 64] tile): SBO = 1024 B between 8-k groups,
+//   LBO = byte stride between 64-element MN chunks; the k-th 16-row K slice starts k * 2048 B into the tile.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor for kind::f16 with fp16 A/B and fp32 accumulate.
-//   bits [4,6) c_format=1 (F32); [7,10) a_format=0 (F16); [10,13) b_format=0 (F16);
-//   bit 15 a_major, bit 16 b_major (0 = K-major, 1 = MN-major); [17,23) N>>3; [24,29) M>>4.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(a_mn_major) << 15) | (static_cast<uint32_t>(b_mn_major) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+// Ordering of the accumulator registers against the asynchronous MMAs of this warpgroup.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Keeps the compiler from moving accumulator reads / writes across an MMA that is still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- CTA-pair (cta_group::2) variants ------------------------------------------------------
-// Two CTAs of a cluster (ranks 2i, 2i+1 — one TPC) cooperate on one MMA: M = 256 rows split 128/128,
-// each CTA stages its A half and half of the B tile; the even ("leader") CTA issues the MMA.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (same smem offset).
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(m), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                 uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] (smem) * B[128 x 16]^T (smem), both K-major; fp16 in, fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// Arrive (once the pair's MMAs retire) on the mbarrier at this smem offset in every CTA of cta_mask.
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
+// D[64 x 64] (+)= A[64 x 16] (smem) * B[64 x 16]^T (smem), both K-major; fp16 in, fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// Same, without release semantics: for hand-offs whose payload is TMEM (ordered by tcgen05.fence) — the default
-// .release.cluster arrive drains the warp's earlier global/shared writes first (~1.6k clk after TMA-store epilogues).
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint64_t* bar, uint32_t cta) {
+// D[64 x 64] (+)= A[64 x 16] (registers: fp16 pairs in the accumulator-fragment order) * B[16 x 64] (smem,
+// MN-major: the 64 columns contiguous, as a row-major [K, N] tile); fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_bmn(float (&d)[32], const uint32_t (&a)[4], uint64_t db,
+                                                       uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-// Arrive on the mbarrier at the same smem offset in CTA `cta` of the cluster.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 
 // ---- misc math ---------------------------------------------------------------------------
@@ -420,10 +299,9 @@ __device__ __forceinline__ float ex2_approx(float x);
 // Exact-erf GELU, 0.5 x (1 + erf(x / sqrt 2)) (timm Mlp / ProjectReadout use nn.GELU()), with erf from
 // 2^x on the FMA/ALU pipes (no MUFU): Cody-Waite split x = n + f, f in [-0.5, 0.5] via the 1.5*2^23 rounding trick,
 // minimax polynomial for 2^f (tools/fit_exp2.py: relative error 7.5e-5 / 2.7e-6 / 2.3e-7 for degree 3 / 4 / 5),
-// exponent added by integer arithmetic on the bit pattern: ~9 issue slots instead of one MUFU instruction (8 clk
-// of the MUFU pipe per warp, tools/probes/mufu_probe.cu). Kept as a measured experiment: neither the attention
-// softmax (LSEG_MHSA_POLY=2|3|4: 64 -> 72-77 us) nor the GELU epilogue got faster — both are bound by issue
-// slots / latency of their few warps, not by MUFU throughput. Requires -126 <= x <= 126 (the callers clamp).
+// exponent added by integer arithmetic on the bit pattern: ~9 issue slots instead of one MUFU instruction. Used by
+// the attention variants that move part of the softmax exponentials off the MUFU pipe (lseg_mhsa_variant 3/4/7/8).
+// Requires -126 <= x <= 126 (the callers clamp).
 template <int DEG>
 __device__ __forceinline__ float exp2_poly(float x) {
   const float r = x + 12582912.f;  // 1.5 * 2^23: the low mantissa bits of r now hold round(x)
@@ -460,8 +338,6 @@ __device__ __forceinline__ float gelu_erf(float x) {
   p = fmaf(p, u, 3.602744768e-04f);
   p = fmaf(p, u, -1.052266877e-01f);
   p = fmaf(p, u, -2.302045391e+00f);
-  // (exp2_poly<4> here instead of the MUFU ex2 was measured SLOWER: fc1 51.8 -> 58.9 us; the epilogue is bound by
-  // issue slots of its 8 warps, not by the MUFU pipe)
   const float e = ex2_approx(x * p);
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));

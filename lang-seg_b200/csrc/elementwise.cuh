@@ -115,8 +115,7 @@ static inline int launch_assemble_tokens(const float* patch, const float* cls, c
 // (SURVEY.md Appendix A.1/A.2). C in {512, 1024} is a template constant (fully unrolled, no predicates).
 // HBM-bound: 6 B per element. A lane owns chunks of 8 consecutive elements (32 B loads in, one 16 B store out per
 // chunk); gamma / beta are staged in shared memory by the whole block while the row loads are in flight, so the
-// normalisation does not wait for a second round trip after the statistics (round 1: 12.5 us for 44 MB, r02: see
-// profiles/r02_layernorm.md).
+// normalisation does not wait for a second round trip after the statistics.
 // ------------------------------------------------------------------------------------------
 template <typename TIn, int C>
 __global__ void __launch_bounds__(256) layernorm_kernel(const TIn* __restrict__ x, const float* __restrict__ gamma,
@@ -428,7 +427,7 @@ __global__ void __launch_bounds__(256, 3) upsample2x_nhwc256_f32_kernel(const fl
   if (ox0 >= Wo) return;
   const float sh = (Ho > 1) ? static_cast<float>(H - 1) / (Ho - 1) : 0.f;
   const float sw = (Wo > 1) ? static_cast<float>(W - 1) / (Wo - 1) : 0.f;
-  const float fy = sh * oy;
+  const float fy = __fmul_rn(sh, oy);  // rounded product, as torch forms the source index (no FMA into ly)
   const int y0 = static_cast<int>(fy);
   const int y1 = min(y0 + 1, H - 1);
   const float ly = fy - y0, hy = 1.f - ly;
@@ -451,7 +450,7 @@ __global__ void __launch_bounds__(256, 3) upsample2x_nhwc256_f32_kernel(const fl
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (ox0 + k >= Wo) break;  // warp-uniform
-      const float fx = sw * (ox0 + k);
+      const float fx = __fmul_rn(sw, ox0 + k);
       const int x0 = static_cast<int>(fx);
       const float lx = fx - x0, hx = 1.f - lx;
       const int d = x0 - xs;  // 0..2, warp-uniform
@@ -492,7 +491,7 @@ __global__ void __launch_bounds__(256, 3) upsample2x_nhwc256_f16_kernel(const __
   if (ox0 >= Wo) return;
   const float sh = (Ho > 1) ? static_cast<float>(H - 1) / (Ho - 1) : 0.f;
   const float sw = (Wo > 1) ? static_cast<float>(W - 1) / (Wo - 1) : 0.f;
-  const float fy = sh * oy;
+  const float fy = __fmul_rn(sh, oy);  // rounded product, as torch forms the source index (no FMA into ly)
   const int y0 = static_cast<int>(fy);
   const int y1 = min(y0 + 1, H - 1);
   const float ly = fy - y0, hy = 1.f - ly;
@@ -512,7 +511,7 @@ __global__ void __launch_bounds__(256, 3) upsample2x_nhwc256_f16_kernel(const __
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (ox0 + k >= Wo) break;  // warp-uniform
-    const float fx = sw * (ox0 + k);
+    const float fx = __fmul_rn(sw, ox0 + k);
     const int x0 = static_cast<int>(fx);
     const float lx = fx - x0, hx = 1.f - lx;
     const int d = x0 - xs;  // 0..2, warp-uniform

@@ -467,7 +467,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
 
 // ResNet-101 trunk of the zero-shot model (lseg_net_zs.py:307-310: pretrained.layer1..4 = torchvision resnet101 stages,
 // lseg_blocks_zs.py:109-119): stem 7x7 s2 (im2col + GEMM, BN + ReLU in the epilogue) -> maxpool -> 33 bottlenecks.
-// Every conv is the tcgen05 GEMM: 1x1 = plain GEMM over the NHWC pixels, 3x3 stride 1 = implicit GEMM, 3x3 stride 2 =
+// Every conv is the wgmma GEMM: 1x1 = plain GEMM over the NHWC pixels, 3x3 stride 1 = implicit GEMM, 3x3 stride 2 =
 // im2col rows + GEMM, 1x1 stride 2 = GEMM over the subsampled pixels; BatchNorm folded into the fp32 epilogue. The
 // residual stream is fp32 (one buffer per stage, updated in place by conv3's epilogue: relu(bn3(conv3) + identity)),
 // with an fp16 copy as the next conv's operand — the same split as the decoder's RCUs.

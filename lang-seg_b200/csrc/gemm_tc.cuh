@@ -1,55 +1,36 @@
-// lseg_b200 — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// lseg_b200 — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   C[M,N] = epilogue( A[M,K] * W[N,K]^T )       fp16 operands, fp32 accumulate in TMEM
+//   C[M,N] = epilogue( A[M,K] * W[N,K]^T )       fp16 operands, fp32 accumulate in registers
 //
 // One kernel family covers every dense contraction of the LSeg forward path (SURVEY.md §2b k1,k4,k6-k8,
 // k10-k17,k19): linear layers, 1x1 convs, kernel==stride transposed convs (depth-to-space store),
 // and 3x3 stride-1 convs as implicit GEMM (the A tile of tap (dy,dx) is a shifted 4-D TMA box of
 // the NHWC activation; TMA zero-fills the padding halo).
 //
-// Roles (one CTA per SM, persistent over a static round-robin tile list):
-//   warp 0   TMA producer       : fills the A/B smem ring (128B-swizzled, K-major)
-//   warp 1   MMA issuer         : tcgen05.mma + commits to mbarriers
-//             (both warps run CONVERGED; one elect.sync lane predicates only the bulk-copy / MMA instructions,
-//              so descriptor arithmetic stays on the uniform datapath — a divergent `if (lane == 0)` region cost
-//              ~20 dependent instructions, ~130 clk, per tcgen05.mma)
-//   warp 2   TMEM allocator
-//   warps 4+ epilogue (8 or 16) : tcgen05.ld accumulator -> regs -> scale/bias/act/residual -> global
-// The accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps
-// the main loop of tile i+1.
+// Roles (one CTA per SM, persistent over a static round-robin list of 128 x 128 tiles):
+//   warpgroup 0   TMA producer (warp 0, one elected lane): fills the A/B smem ring (128B-swizzled, K-major)
+//   warpgroups 1-2  consumers: each issues wgmma m64n128k16 for 64 of the tile's 128 rows (accumulator in registers),
+//                 then stages its fp32 accumulators in shared memory, and the 8 consumer warps run the epilogue with
+//                 thread <-> output row (warp = 32 rows x 64 columns): scale/bias/act/residual -> global.
+// The producer runs up to kStages k-chunks ahead, so the next tile's operands stream in during the epilogue.
 //
-// Kernels
-//   gemm_tc2_kernel<BN, EPI, EW>  CTA pair (tcgen05 cta_group::2, UMMA 256 x BN x 16): default. Shared-memory
-//        bandwidth is the binding resource of an SS-mode UMMA main loop (every byte TMA writes is read back by
-//        the tensor core); the pair splits the weight tile, so each SM stages 32 KB per k-step instead of 48.
-//
-// Epilogue modes (measured with tools/gemm_probe.py / tools/gemm_trace.py: the main loop alone runs at
-// 1450-1500 TFLOP/s on the ViT shapes, so for K <= 1024 the epilogue decides the speed; with the tensor core
-// writing the other accumulator buffer a tcgen05.ld returns after ~700 clk):
-//   EPI_DIRECT   stores straight from registers, thread <-> accumulator row. Every 16 B access of a warp
-//                touches 32 different 128 B lines = 32 L1TEX wavefronts; fine for long-K tiles, 2-3x the
-//                main-loop time for K = 1024.
+// Epilogue modes:
+//   EPI_DIRECT   stores straight from registers, thread <-> accumulator row.
 //   EPI_TMA_F16  fp16 row-major outputs: each epilogue warp packs 32 rows x 64 columns into a private
-//                128B-swizzled smem tile and one elected lane issues a bulk tensor store (QKV 58 -> 36 us);
-//                EW = 16 epilogue warps (64 columns each, one staging tile per warp) where K <= 512 or GELU.
+//                128B-swizzled smem tile and one elected lane issues a bulk tensor store.
 //   EPI_TMA_ADD  in-place fp32 residual stream (x += A W^T + b): the warp stages 32 x 32 fp32 results and
 //                issues a bulk tensor REDUCE-ADD, so the residual is never read by the SM at all.
-// Per-column constants (bias, folded-BN scale) live in registers per tile and are distributed by shuffle; the
-// TMEM hand-off back to the MMA warp is a relaxed cluster arrive (a release arrive drains the stores: 1.6k clk).
-// Rejected after measurement: a full smem transpose of the accumulator (competes with the main loop for smem
-// bandwidth: every GEMM 1.3-2.3x slower) and computing D^T so that lanes map to columns (4 B accesses: 4x
-// the LSU instructions, proj 39 -> 84 us).
+// Per-column constants (bias, folded-BN scale) live in registers per tile and are distributed by shuffle.
 #pragma once
 #include "common.cuh"
 
 namespace lseg {
 
 constexpr int kGemmBM = 128;
+constexpr int kGemmBN = 128;
 constexpr int kGemmBK = 64;
 constexpr int kConvTH = 8;   // conv M tile = 8 x 16 output pixels
 constexpr int kConvTW = 16;
-constexpr int kGemmEpiWarps = 8;
-constexpr int kGemmThreads = 128 + 32 * kGemmEpiWarps;
 
 enum GemmAct { ACT_NONE = 0, ACT_GELU = 1, ACT_QUICKGELU = 2, ACT_RELU = 3 };
 enum GemmStore { STORE_ROWMAJOR = 0, STORE_D2S = 1, STORE_NCHW_T = 2 };
@@ -93,17 +74,17 @@ struct GemmParams {
   int H, W, kw, pad;
   int tiles_h, tiles_w;
   int num_m_tiles, num_n_tiles;
-  int split_k;   // EPI_TMA_ADD only: balance (tile, k-chunk) units over the CTA pairs instead of whole tiles
+  int split_k;   // EPI_TMA_ADD only: balance (tile, k-chunk) units over the CTAs instead of whole tiles
   int split_fixed;       // EPI_DIRECT, >= 2: every tile's K loop is cut into this many equal segments, each a work unit of
   long long split_rows;  //   its own; segment s stores its RAW fp32 partial at row (s * split_rows + row) of out_f32 and
                          //   splitk_reduce_kernel sums the segments in index order (deterministic) and applies the epilogue
-  unsigned long long* trace;  // debug timeline ([2 pairs][12 warps][512] of clock64 << 8 | tag), normally nullptr
-  int probe;  // measurement only (tools/gemm_probe.py; results are garbage when non-zero):
-              //   1 = skip epilogue work, 2 = skip TMA loads, 4 = skip MMA issue   (CTA-pair kernel)
+  unsigned long long* trace;  // debug timeline ([2 CTAs][20 warps][512] of clock64 << 8 | tag), normally nullptr
+  int probe;  // measurement only (results are garbage when non-zero):
+              //   1 = skip epilogue work, 2 = skip TMA loads, 4 = skip MMA issue
   GemmEpi e;
 };
 
-// Debug timeline of one warp (tools/gemm_trace.py): stamps are dropped when w == nullptr (always, outside the tool).
+// Debug timeline of one warp (lseg_debug_gemm_trace): stamps are dropped when w == nullptr (always, unless enabled).
 // The stamp itself is an out-of-line call so that the untraced kernel pays one predicated branch per site, not a
 // predicated copy of the stamp code.
 __device__ __noinline__ int gemm_trace_stamp(unsigned long long* w, int n, int tag) {
@@ -124,8 +105,7 @@ struct GemmTrace {
 // ------------------------------------------------------------------------------------------
 // Per-column constants of the (up to) 128 columns a warp handles in one tile, held in registers: lane l keeps
 // columns 4l..4l+3 (zeros beyond N), fetched with ONE coalesced 16-byte load per lane before the accumulator is
-// even awaited; chunk c then takes them by shuffle. The per-chunk global loads this replaces cost ~700 clk of
-// exposed latency per 32-column chunk (profiles: tools/gemm_trace.py), the largest single item of the epilogue.
+// even awaited; chunk c then takes them by shuffle instead of issuing dependent global loads per 32-column chunk.
 struct GemmColConst {
   float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
   float4 scale = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -360,11 +340,24 @@ __device__ __forceinline__ bool gemm_row_map(const GemmParams& p, int m_tile, in
 
 constexpr int kEpiStageBytes = 2 * 4096;  // per epilogue warp: two 32-row x 128 B swizzled tiles (TMA epilogues)
 
-// Epilogue of one 128 x (ncols) accumulator slab for one warp (r = quarter*32 + lane = this thread's row).
-// SINGLE_BUF: one 4 KB staging tile per warp instead of two (16-epilogue-warp configuration, where a warp emits one
-// store group per tile and the previous tile's bulk store has long finished reading the buffer).
+// 32 consecutive fp32 accumulators of one row of the staged tile (16-byte aligned)
+__device__ __forceinline__ void gemm_acc_ld32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 q = reinterpret_cast<const float4*>(src)[i];
+    v[4 * i] = __float_as_uint(q.x);
+    v[4 * i + 1] = __float_as_uint(q.y);
+    v[4 * i + 2] = __float_as_uint(q.z);
+    v[4 * i + 3] = __float_as_uint(q.w);
+  }
+}
+
+// Epilogue of one 128 x (ncols) accumulator slab for one warp (r = quarter*32 + lane = this thread's row); acc_row is
+// this thread's row of the fp32 accumulator tile staged in shared memory, at the warp's first column.
+// SINGLE_BUF: one 4 KB staging tile per warp instead of two (leaves the shared memory to the accumulator tile and the
+// operand ring; the warp then waits for its previous bulk store to finish reading before it refills the buffer).
 template <int EPI, bool SINGLE_BUF = false, bool GROUPED = false, bool RELU_RES = false, typename WaitFn>
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t t_row, int n_base, int ncols,
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc_row, int n_base, int ncols,
                                                    int m_tile, int r, WaitFn wait_accumulator, uint8_t* stage_buf,
                                                    int& store_groups, GemmTrace& tr, bool first_k = true,
                                                    int split_seg = 0) {
@@ -396,7 +389,6 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t
       row_mul = e.row_scale * rsqrtf(ss);
     }
     wait_accumulator();
-    tc_fence_after();
     if (p.probe & 1) return;
 #pragma unroll 1
     for (int c = 0; c < ncols / 32; ++c) {
@@ -413,8 +405,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t
       }
       uint32_t v[32];
       __syncwarp();
-      tmem_ld32(t_row + c * 32, v);
-      tmem_ld_wait();
+      gemm_acc_ld32(acc_row + c * 32, v);
       float f[32];
       gemm_epilogue_math(e, p.N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
       if (valid) {
@@ -441,7 +432,6 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t
     const GemmColConst cc = gemm_col_const(e, p.N, n_base, ncols, lane);
     const bool leader = elect_one_sync();  // issues (and owns the bulk groups of) this warp's TMA stores
     wait_accumulator();
-    tc_fence_after();
     tr(1);
     if (p.probe & 1) return;
     int groups = store_groups;
@@ -451,8 +441,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t
       if (n0 >= p.N) break;  // warp-uniform
       uint32_t v[32];
       __syncwarp();
-      tmem_ld32(t_row + c * 32, v);
-      tmem_ld_wait();
+      gemm_acc_ld32(acc_row + c * 32, v);
       tr(2);
       float f[32];
       gemm_epilogue_math(e, p.N, v, grow_c, n0, bias_off, valid, f, cc, c, first_k);
@@ -516,64 +505,48 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, uint32_t
 }
 
 // ==========================================================================================
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs (one TPC) computes a 256 x BN tile.
-// Each CTA stages its own 128 A rows and HALF of the weight tile; the even CTA issues
-// tcgen05.mma.cta_group::2 (M = 256) for the pair; both CTAs run a TMA producer and 8 epilogue warps
-// over their own 128 TMEM lanes.
-//   full barrier   : in the leader, armed with the pair's byte count; both CTAs' TMA credit it
-//   empty barrier  : per CTA, released by a multicast tcgen05.commit
-//   tmem full      : per CTA (multicast commit);  tmem empty: in the leader, 2 x 8 warp arrivals
+// The kernel: persistent CTAs over 128 x 128 output tiles (warp roles in the header comment).
+//   full barrier  : per stage, armed by the producer with the stage's byte count; the TMA loads credit it
+//   empty barrier : per stage, one arrival per consumer warp once its warpgroup's MMAs have read the stage
 // ==========================================================================================
-template <int BN, int EPI, int EW = 8>
-struct Gemm2Cfg {
-  static constexpr int kABytes = kGemmBM * kGemmBK * 2;
-  static constexpr int kBBytes = (BN / 2) * kGemmBK * 2;  // this CTA's half of the weight tile
+template <int EPI>
+struct GemmCfg {
+  static constexpr int kABytes = kGemmBM * kGemmBK * 2;  // 16 KB
+  static constexpr int kBBytes = kGemmBN * kGemmBK * 2;  // 16 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // Epilogue warps EW: 8, or 16 (fp16 TMA-store epilogue of 256-wide tiles only: 4 warps per TMEM lane quarter, 64
-  // columns each). The planner picks 16 where the epilogue, not the main loop, bounds the tile — K <= 512 (head1
-  // 251 -> 185 us, 1x1 out_conv 110 -> 87 us) and the GELU epilogue of fc1 (61 -> 58 us); with long K the extra
-  // warps only take issue slots from the producer / MMA warps (QKV +2 us, 3x3 convs +6 us).
-  static_assert(EW == 8 || (EW == 16 && EPI == EPI_TMA_F16 && BN == 256), "16 epilogue warps: TMA fp16 store, BN 256");
-  static constexpr int kEpiWarps = EW;
-  static constexpr int kThreads = 128 + 32 * kEpiWarps;
-  static constexpr int kEpiBufBytes = (kEpiWarps == 16) ? 4096 : kEpiStageBytes;
-  // stages | per-warp TMA-epilogue staging (1024 B aligned) | mbarriers
+  static constexpr int kEpiWarps = 8;                     // the two consumer warpgroups
+  static constexpr int kThreads = 128 + 32 * kEpiWarps;   // + the producer warpgroup
+  static constexpr int kEpiBufBytes = 4096;               // one 32-row x 128 B TMA-store staging tile per warp
   static constexpr int kStageOutBytes = (EPI == EPI_DIRECT) ? 0 : kEpiWarps * kEpiBufBytes;
-  // BN = 224 (in-place residual GEMMs with N = 1024: 5 tiles of 224 make 145 pair tiles = 1.96 waves of 74 CTA pairs
-  // where 4 tiles of 256 make 116 = 1.57 -> 2 waves of wider tiles) shares the BN = 256 pipeline depth.
-  static constexpr int kStages = (BN >= 224) ? ((EPI == EPI_DIRECT) ? 6 : 5) : ((EPI == EPI_DIRECT) ? 8 : 6);
-  static constexpr int kTmemCols = (2 * BN <= 256) ? 256 : 512;  // tcgen05.alloc takes powers of two
-  // columns of the 8-warp epilogue's first column half (a multiple of 32); the second half takes the rest
-  static constexpr int kColsHalf0 = ((BN / 2 + 31) / 32) * 32;
-  static_assert(BN % 32 == 0 && BN % 16 == 0 && BN <= 256, "tile width");
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + 1024 + 256;
+  static constexpr int kAccStride = kGemmBN + 4;          // fp32 row stride of the staged accumulators (bank spread)
+  static constexpr int kAccBytes = kGemmBM * kAccStride * 4;
+  // operand ring | per-warp TMA-store staging (1024 B aligned) | accumulator tile | mbarriers: <= 227 KB
+  static constexpr int kStages = (EPI == EPI_DIRECT) ? 4 : 3;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + kAccBytes + 1024 + 256;
 };
 
-// FIXED_SPLIT: the deterministic split-K schedule (GemmParams::split_fixed) is its own instantiation — its index
-// arithmetic costs the other kernels their uniform-datapath code (UISETP 254 -> 97, BSSY/BSYNC pairs appear) when it is
-// merely present as a runtime branch.
-template <int BN, int EPI, int EW = 8, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((Gemm2Cfg<BN, EPI, EW>::kThreads), 1)
-    gemm_tc2_kernel(const __grid_constant__ GemmParams p) {
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// FIXED_SPLIT: the deterministic split-K schedule (GemmParams::split_fixed) is its own instantiation, so its index
+// arithmetic stays out of the other kernels.
+template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false>
+__global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   static_assert(!RELU_RES || (EPI == EPI_DIRECT && !FIXED_SPLIT && !GROUPED), "relu-after-residual: plain register-direct");
   static_assert(!FIXED_SPLIT || EPI == EPI_DIRECT, "split-K partials leave through the register-direct epilogue");
   static_assert(!GROUPED || (EPI == EPI_DIRECT && !FIXED_SPLIT), "per-image column blocks: NCHW-T store, register-direct");
-  using Cfg = Gemm2Cfg<BN, EPI, EW>;
+  using Cfg = GemmCfg<EPI>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_out = smem + Cfg::kStages * Cfg::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_out + Cfg::kStageOutBytes);
+  float* acc_tile = reinterpret_cast<float*>(stage_out + Cfg::kStageOutBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_tile) + Cfg::kAccBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tmem_full = bars + 2 * Cfg::kStages;
-  uint64_t* tmem_empty = bars + 2 * Cfg::kStages + 2;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::kStages + 4);
 
   const int warp = warp_idx_sync();  // provably warp-uniform: role branches and their operands stay on the uniform datapath
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();  // 0 = leader
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
+  const int cta = blockIdx.x;
+  const int num_ctas = gridDim.x;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tma_a);
@@ -581,29 +554,19 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((Gemm2Cfg<BN, EPI, E
     if (EPI != EPI_DIRECT) tma_prefetch_desc(&p.tma_c);
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 2 * Cfg::kEpiWarps);
+      mbar_init(&empty_bar[i], Cfg::kEpiWarps);
     }
     mbar_fence_init();
   }
   griddep_launch_dependents();
-  if (warp == 2) tmem_alloc_2cta(tmem_base_slot, Cfg::kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();  // barriers + TMEM of BOTH CTAs exist before any cross-CTA traffic
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
+  __syncthreads();
   griddep_wait();  // everything above overlapped the previous kernel's tail; operands / outputs are touched below
 
-  const int m_pairs = (p.num_m_tiles + 1) >> 1;
-  const int num_tiles = m_pairs * p.num_n_tiles;  // pair tiles (256 x BN)
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
-  // Work schedule of this CTA pair. Default: whole 256 x BN tiles, pair, pair + P, ... . split_k (in-place residual
-  // GEMMs only, whose epilogue is a reduce-add and therefore composes over partial sums): the (tile, k-chunk) units
-  // are dealt out evenly, so a pair handles a contiguous range that may start / end inside a tile — 116 tiles on 74
-  // pairs are 2 waves of whole tiles but only 1.57 tiles of work per pair. The bias is added by the k = 0 segment.
+  // Work schedule of this CTA. Default: whole tiles cta, cta + G, ... . split_k (in-place residual GEMMs only, whose
+  // epilogue is a reduce-add and therefore composes over partial sums): the (tile, k-chunk) units are dealt out evenly,
+  // so a CTA handles a contiguous range that may start / end inside a tile. The bias is added by the k = 0 segment.
   struct Sched {
     int tile_next, tile_step, num_tiles, k_iters;
     long long unit, unit_end;
@@ -638,8 +601,8 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((Gemm2Cfg<BN, EPI, E
   };
   auto make_sched = [&]() {
     Sched sc;
-    sc.tile_next = pair;
-    sc.tile_step = num_pairs;
+    sc.tile_next = cta;
+    sc.tile_step = num_ctas;
     sc.num_tiles = num_tiles;
     sc.k_iters = p.k_iters;
     sc.split = (EPI == EPI_TMA_ADD) && p.split_k;
@@ -647,157 +610,138 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((Gemm2Cfg<BN, EPI, E
     sc.seg = 0;
     const long long units = static_cast<long long>(num_tiles) * p.k_iters;
     // boundaries on multiples of 4 k-chunks: no sliver segments whose epilogue would cost more than their MMAs
-    sc.unit = ((units * pair / num_pairs) + 3) & ~3ll;
-    sc.unit_end = (pair + 1 == num_pairs) ? units : (((units * (pair + 1) / num_pairs) + 3) & ~3ll);
+    sc.unit = ((units * cta / num_ctas) + 3) & ~3ll;
+    sc.unit_end = (cta + 1 == num_ctas) ? units : (((units * (cta + 1) / num_ctas) + 3) & ~3ll);
     if (sc.unit_end > units) sc.unit_end = units;
     return sc;
   };
 
   if (warp == 0) {
-    // ===================== TMA producer (both CTAs; converged warp, elected issuing lane) =====================
-    {
-      const bool leader = elect_one_sync();
-      int stage = 0;
-      uint32_t phase = 0;
-      Sched sc = make_sched();
-      int tile, k_begin, k_end;
-      while (sc.next(tile, k_begin, k_end)) {
-        const int m_tile = (tile % m_pairs) * 2 + static_cast<int>(rank);
-        const int n_tile = tile / m_pairs;
-        const int n0 = n_tile * BN + static_cast<int>(rank) * (BN / 2);
-        int cb = 0, ch0 = 0, cw0 = 0;
-        if (p.conv) {
-          const int per_img = p.tiles_h * p.tiles_w;
-          cb = m_tile / per_img;  // == B for the phantom tile of an odd count -> TMA zero-fills
-          const int t = m_tile % per_img;
-          ch0 = (t / p.tiles_w) * kConvTH;
-          cw0 = (t % p.tiles_w) * kConvTW;
-        }
-        for (int kit = k_begin; kit < k_end; ++kit) {
-          mbar_wait(&empty_bar[stage], phase ^ 1, 21);
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
-          if (p.probe & 2) {
-            if (rank == 0 && leader) mbar_arrive(&full_bar[stage]);
-            __syncwarp();
-            if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-            continue;
-          }
-          int c0 = kit * kGemmBK, c1 = m_tile * kGemmBM, c2 = 0;
-          if (p.conv) {
-            const int tap = kit / p.k_chunks;
-            const int c = kit - tap * p.k_chunks;
-            const int dy = tap / p.kw, dx = tap - dy * p.kw;
-            c0 = c * kGemmBK;
-            c1 = cw0 + dx - p.pad;
-            c2 = ch0 + dy - p.pad;
-          }
-          if (leader) {
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-            if (p.conv)
-              tma_load_4d_2sm(sa, &p.tma_a, &full_bar[stage], c0, c1, c2, cb);
-            else
-              tma_load_2d_2sm(sa, &p.tma_a, &full_bar[stage], c0, c1);
-            tma_load_2d_2sm(sb, &p.tma_b, &full_bar[stage], kit * kGemmBK, n0);
-          }
-          __syncwarp();
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only; converged warp, elected issuing lane) =====================
-    if (rank == 0) {
-      const bool leader = elect_one_sync();
-      constexpr uint32_t idesc = umma_idesc_f16(2 * kGemmBM, BN, 0, 0);
-      GemmTrace tr;
-      if (p.trace && lane == 0 && (pair == 0 || pair == num_pairs / 2)) tr.w = p.trace + ((pair == 0 ? 0 : 1) * 20 + warp) * 512;
-      tr(0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      Sched sc = make_sched();
-      int tile, k_begin, k_end;
-      while (sc.next(tile, k_begin, k_end)) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1, 22);
-        tc_fence_after();
-        tr(10);
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kit = k_begin; kit < k_end; ++kit) {
-          mbar_wait(&full_bar[stage], phase, 23);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t b_base = a_base + Cfg::kABytes;
-          if (leader) {
-            if (!(p.probe & 4)) {
-#pragma unroll
-              for (int k = 0; k < kGemmBK / 16; ++k) {
-                const uint64_t da = umma_desc_sw128(a_base + k * 32, 1024, 0);
-                const uint64_t db = umma_desc_sw128(b_base + k * 32, 1024, 0);
-                umma_f16_ss_2cta(d_tmem, da, db, idesc, (kit != k_begin) || (k != 0));
-              }
-            }
-            umma_commit_2cta(&empty_bar[stage], 0x3);  // both CTAs' smem slots
-          }
-          __syncwarp();
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        if (leader) umma_commit_2cta(&tmem_full[acc], 0x3);
-        __syncwarp();
-        tr(12);
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== Epilogue (both CTAs, own 128 TMEM lanes) =====================
-    const int ew = warp - 4;
-    const int quarter = warp & 3;
-    const int half = ew >> 2;
-    // 8 warps: two column halves (kColsHalf0 | BN - kColsHalf0); 16 warps: four quarters of BN / 4
-    constexpr int kColsPerWarp = BN / (Cfg::kEpiWarps / 4);
-    const int col0 = (Cfg::kEpiWarps == 16) ? half * kColsPerWarp : half * Cfg::kColsHalf0;
-    const int ncols = (Cfg::kEpiWarps == 16) ? kColsPerWarp : (half == 0 ? Cfg::kColsHalf0 : BN - Cfg::kColsHalf0);
-    const int r = quarter * 32 + lane;
-    uint8_t* stage_buf = stage_out + ew * Cfg::kEpiBufBytes;
-    int store_groups = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    GemmTrace tr;
-    if (p.trace && lane == 0 && rank == 0 && (pair == 0 || pair == num_pairs / 2))
-      tr.w = p.trace + ((pair == 0 ? 0 : 1) * 20 + warp) * 512;
-    tr(0);
+    // ===================== TMA producer (converged warp, elected issuing lane) =====================
+    const bool leader = elect_one_sync();
+    int stage = 0;
+    uint32_t phase = 0;
     Sched sc = make_sched();
     int tile, k_begin, k_end;
     while (sc.next(tile, k_begin, k_end)) {
-      const int m_tile = (tile % m_pairs) * 2 + static_cast<int>(rank);
-      const int n_tile = tile / m_pairs;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + col0;
-      gemm_epilogue_tile<EPI, Cfg::kEpiWarps == 16, GROUPED, RELU_RES>(p, t_row, n_tile * BN + col0, ncols, m_tile, r,
-                              [&]() { mbar_wait(&tmem_full[acc], acc_phase, 24); }, stage_buf, store_groups, tr,
-                              k_begin == 0, FIXED_SPLIT ? sc.seg : 0);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster_relaxed(&tmem_empty[acc], 0);  // leader CTA's barrier: 2 CTAs x 8 warps
+      const int m_tile = tile % p.num_m_tiles;
+      const int n0 = (tile / p.num_m_tiles) * kGemmBN;
+      int cb = 0, ch0 = 0, cw0 = 0;
+      if (p.conv) {
+        const int per_img = p.tiles_h * p.tiles_w;
+        cb = m_tile / per_img;
+        const int t = m_tile % per_img;
+        ch0 = (t / p.tiles_w) * kConvTH;
+        cw0 = (t % p.tiles_w) * kConvTW;
+      }
+      for (int kit = k_begin; kit < k_end; ++kit) {
+        mbar_wait(&empty_bar[stage], phase ^ 1, 21);
+        uint8_t* sa = smem + stage * Cfg::kStageBytes;
+        uint8_t* sb = sa + Cfg::kABytes;
+        if (p.probe & 2) {
+          if (leader) mbar_arrive(&full_bar[stage]);
+          __syncwarp();
+          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+          continue;
+        }
+        int c0 = kit * kGemmBK, c1 = m_tile * kGemmBM, c2 = 0;
+        if (p.conv) {
+          const int tap = kit / p.k_chunks;
+          const int c = kit - tap * p.k_chunks;
+          const int dy = tap / p.kw, dx = tap - dy * p.kw;
+          c0 = c * kGemmBK;
+          c1 = cw0 + dx - p.pad;
+          c2 = ch0 + dy - p.pad;
+        }
+        if (leader) {
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          if (p.conv)
+            tma_load_4d(sa, &p.tma_a, &full_bar[stage], c0, c1, c2, cb);
+          else
+            tma_load_2d(sa, &p.tma_a, &full_bar[stage], c0, c1);
+          tma_load_2d(sb, &p.tma_b, &full_bar[stage], kit * kGemmBK, n0);
+        }
+        __syncwarp();
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================== consumers: MMA main loop, then the epilogue =====================
+    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile in the main loop
+    const int wl = warp & 3;         // warp within its warpgroup: accumulator rows 16 wl .. 16 wl + 15
+    const int ew = warp - 4;
+    const int quarter = ew & 3;      // epilogue: rows [32 quarter, +32), columns [64 half, +64)
+    const int half = ew >> 2;
+    const int r = quarter * 32 + lane;
+    const int col0 = half * 64;
+    const float* acc_row = acc_tile + r * Cfg::kAccStride + col0;
+    uint8_t* stage_buf = stage_out + ew * Cfg::kEpiBufBytes;
+    int store_groups = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    GemmTrace tr;
+    if (p.trace && lane == 0 && (cta == 0 || cta == num_ctas / 2)) tr.w = p.trace + ((cta == 0 ? 0 : 1) * 20 + warp) * 512;
+    tr(0);
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    Sched sc = make_sched();
+    int tile, k_begin, k_end;
+    while (sc.next(tile, k_begin, k_end)) {
+      const int m_tile = tile % p.num_m_tiles;
+      const int n_tile = tile / p.num_m_tiles;
+      int prev = -1;
+      for (int kit = k_begin; kit < k_end; ++kit) {
+        mbar_wait(&full_bar[stage], phase, 23);
+        __syncwarp();
+        const uint32_t a_base = smem_u32(smem + stage * Cfg::kStageBytes) + wg * (64 * 128);
+        const uint32_t b_base = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
+        if (!(p.probe & 4)) {
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kGemmBK / 16; ++k)
+            wgmma_m64n128k16_ss(acc, wgmma_desc_sw128(a_base + k * 32, 1024, 16),
+                                wgmma_desc_sw128(b_base + k * 32, 1024, 16), (kit != k_begin) || (k != 0));
+          wgmma_commit();
+        }
+        wgmma_wait<1>();  // the previous chunk's MMAs have read their stage: hand it back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      tr(12);
+      // stage the accumulators (fragment rows 64 wg + 16 wl + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) once the
+      // previous tile's epilogue has read the tile
+      consumer_bar_sync();
+      {
+        float* d0 = acc_tile + (wg * 64 + wl * 16 + (lane >> 2)) * Cfg::kAccStride + 2 * (lane & 3);
+        float* d1 = d0 + 8 * Cfg::kAccStride;
+#pragma unroll
+        for (int j = 0; j < kGemmBN / 8; ++j) {
+          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(d1 + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      // the next tile's first MMA ignores the accumulator (scale-d = 0): dead values, not 64 registers held across the
+      // epilogue
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      consumer_bar_sync();
+      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN + col0, 64, m_tile, r, []() {},
+                                                       stage_buf, store_groups, tr, k_begin == 0,
+                                                       FIXED_SPLIT ? sc.seg : 0);
       tr(7);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
     if (EPI != EPI_DIRECT && elect_one_sync()) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // no CTA may exit (or free TMEM) while its peer can still touch it
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, Cfg::kTmemCols);
   }
 }
 
 // ------------------------------------------------------------------------------------------
 // Deterministic split-K, second half: out = epilogue(sum_s partial[s]) for the GEMMs whose tile count leaves most of
-// the CTA pairs idle (3x3 convs on the 15x15 / 30x30 decoder levels: 8 and 29 pair tiles on 74 pairs, K up to 9216).
+// the CTAs idle (3x3 convs on the 15x15 decoder level, K up to 9216).
 // ws fp32 [S][M][N] (N == ldc of the partials); one thread = 4 consecutive columns of one row, segments summed in index
 // order. Epilogue = the row-major subset of gemm_epilogue_math / gemm_epilogue_store: scale, bias (per column), act, two
 // fp32 residuals, fp32 / fp16 / relu-fp16 outputs with the FINAL row stride e.ldc.

@@ -1,5 +1,5 @@
 // lseg_b200 — single translation unit of liblseg_b200.so: host launchers, the C ABI declared in
-// include/lseg_b200.h, and (engine.cuh) the whole-model forward. Compiled for sm_100a only.
+// include/lseg_b200.h, and (engine.cuh) the whole-model forward. Compiled for sm_90a only.
 #include "../../include/lseg_b200.h"
 
 #include <stdarg.h>
@@ -14,9 +14,6 @@
 #include "elementwise.cuh"
 #include "gemm_tc.cuh"
 #include "mhsa.cuh"
-#include "mhsa2.cuh"
-#include "mhsa3.cuh"
-#include "mhsa4.cuh"
 #include "text_attn.cuh"
 #include "p2p.cuh"
 #include "evaluator.cuh"
@@ -42,14 +39,12 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static PFN_encodeTiled g_encode = nullptr;
-static int g_num_sms = 0;        // SM count of the devices this process uses (all must agree: B200 = 148)
-static int g_gemm_two_cta = 1;
+static int g_num_sms = 0;        // SM count of the devices this process uses (all must agree: H100 SXM = 132)
 static int g_deterministic = 1;  // 1 (default): fixed summation order; 0: split-K allowed (LSEG_SPLITK=1 / lseg_set_deterministic(0))
 static int g_plan_epoch = 0;     // bumped when an option that is baked into cached plans changes
 static unsigned long long* g_gemm_trace = nullptr;  // debug (lseg_debug_gemm_trace)
 static int g_gemm_probe = 0;
-static int g_mhsa_variant = 0;   // kernel the engine's ViT attention runs (lseg_mhsa_variant documents the numbering;
-                                 // 1..8 measured within +-3 % of 0 in the step, profiles/r02_mhsa_analysis.md)
+static int g_mhsa_variant = 0;   // kernel the engine's ViT attention runs (lseg_mhsa_variant documents the numbering)
 static std::mutex g_init_mutex;
 static bool g_global_init = false;
 constexpr int kMaxDevices = 64;
@@ -81,8 +76,8 @@ static int init_device(int dev) {
     set_error("lseg_b200: cudaGetDeviceProperties failed");
     return -1;
   }
-  if (prop.major != 10) {
-    set_error("lseg_b200: device '%s' is sm_%d%d; this library contains sm_100a code only", prop.name, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("lseg_b200: device '%s' is sm_%d%d; this library contains sm_90a code only", prop.name, prop.major,
               prop.minor);
     return -1;
   }
@@ -92,49 +87,19 @@ static int init_device(int dev) {
     return -1;
   }
   g_num_sms = prop.multiProcessorCount;
-#define LSEG_SET_SMEM_TC2(BN_, EPI_)                                                             \
-  cudaFuncSetAttribute(gemm_tc2_kernel<BN_, EPI_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                       Gemm2Cfg<BN_, EPI_>::kSmemBytes)
-  LSEG_SET_SMEM_TC2(256, EPI_DIRECT);
-  LSEG_SET_SMEM_TC2(256, EPI_TMA_F16);
-  LSEG_SET_SMEM_TC2(256, EPI_TMA_ADD);
-  LSEG_SET_SMEM_TC2(128, EPI_DIRECT);
-  LSEG_SET_SMEM_TC2(128, EPI_TMA_F16);
-  LSEG_SET_SMEM_TC2(128, EPI_TMA_ADD);
-  LSEG_SET_SMEM_TC2(224, EPI_TMA_ADD);
-#undef LSEG_SET_SMEM_TC2
-  cudaFuncSetAttribute(gemm_tc2_kernel<256, EPI_DIRECT, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<128, EPI_DIRECT, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<256, EPI_DIRECT, 8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<128, EPI_DIRECT, 8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<256, EPI_DIRECT, 8, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<128, EPI_DIRECT, 8, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes);
-  cudaFuncSetAttribute(gemm_tc2_kernel<256, EPI_TMA_F16, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       Gemm2Cfg<256, EPI_TMA_F16, 16>::kSmemBytes);
-#define LSEG_M2_ATTR(K)                                                                       \
-  cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, kM2SmemBytes);          \
-  cudaFuncSetAttribute(K, cudaFuncAttributePreferredSharedMemoryCarveout, 100)
-  LSEG_M2_ATTR((mhsa2_kernel<0, false>));
-  LSEG_M2_ATTR((mhsa2_kernel<kMhsaPolyDefault, true>));
-  LSEG_M2_ATTR((mhsa3_kernel<false, 0>));
-  LSEG_M2_ATTR((mhsa3_kernel<true, 0>));
-  LSEG_M2_ATTR((mhsa3_kernel<true, 1>));
-  LSEG_M2_ATTR((mhsa3_kernel<true, 2>));
-#undef LSEG_M2_ATTR
-#define LSEG_M4_ATTR(K)                                                                       \
-  cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, kM4SmemBytes);          \
-  cudaFuncSetAttribute(K, cudaFuncAttributePreferredSharedMemoryCarveout, 100)
-  LSEG_M4_ATTR((mhsa4_kernel<false, 0>));
-  LSEG_M4_ATTR((mhsa4_kernel<true, 0>));
-  LSEG_M4_ATTR((mhsa4_kernel<true, 1>));
-  LSEG_M4_ATTR((mhsa4_kernel<true, 2>));
-#undef LSEG_M4_ATTR
+#define LSEG_SET_SMEM(KERNEL, EPI_) \
+  cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<EPI_>::kSmemBytes)
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT>), EPI_DIRECT);
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_TMA_F16>), EPI_TMA_F16);
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_TMA_ADD>), EPI_TMA_ADD);
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT);
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT);
+  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT);
+#undef LSEG_SET_SMEM
+  cudaFuncSetAttribute(mhsa_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
+  cudaFuncSetAttribute(mhsa_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
+  cudaFuncSetAttribute(mhsa_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
+  cudaFuncSetAttribute(mhsa_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   if (cudaGetLastError() != cudaSuccess) {
     set_error("lseg_b200: cudaFuncSetAttribute failed on device %d", dev);
     return -1;
@@ -213,38 +178,35 @@ int read_watchdog(int out[4], cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 struct GemmPlan {
   GemmParams p;
-  int bn;
   int grid;
-  int ew16;     // 1: 16 epilogue warps (short-K / GELU fp16 TMA-store GEMMs)
-  int two_cta;  // 1: CTA-pair kernel (tcgen05 cta_group::2), 0: single-CTA kernel
-  int epi;      // GemmEpiMode (CTA-pair kernel)
+  int epi;      // GemmEpiMode
   // deterministic split-K (gemm_tc.cuh splitk_reduce_kernel): p.split_fixed segments per tile write raw partials to a
   // workspace the CALLER provides (gemm_set_workspace) before gemm_run; final_epi is the epilogue the reduce applies
   size_t ws_bytes;
   GemmEpi final_epi;
 };
 
-// Split the K loop of the implicit-GEMM convs whose tile count leaves most CTA pairs idle (3x3 convs on the 15x15 / 30x30
-// decoder levels, layer3_rn / layer4_rn). The segment count is a function of the PER-IMAGE geometry only — it is sized
+// Split the K loop of the implicit-GEMM convs whose tile count leaves most CTAs idle (3x3 convs on the 15x15 decoder
+// level, layer4_rn). The segment count is a function of the PER-IMAGE geometry only — it is sized
 // for a batch of kSplitRefBatch images whatever the actual batch — so the summation order, and with it every bit of the
 // result, is the same for batch 1 and batch 64 (the evaluator's batched and one-by-one runs must agree exactly).
 constexpr int kSplitRefBatch = 8;
-static int gemm_pick_split(const GemmDesc& d, const GemmParams& p, int n_tiles, int max_pairs) {
+static int gemm_pick_split(const GemmDesc& d, const GemmParams& p, int n_tiles, int max_ctas) {
   static const int mode = getenv("LSEG_SPLITK_FIXED") ? atoi(getenv("LSEG_SPLITK_FIXED")) : -1;  // 0 off, >1 forced, -1 auto
-  if (mode == 0 || !g_gemm_two_cta || !d.conv) return 0;
+  if (mode == 0 || !d.conv) return 0;
   const GemmEpi& e = d.e;
   const bool plain_epi = e.store == STORE_ROWMAJOR && e.bias_group_rows == 0 && !e.out_row_sumsq && !e.res_f16 &&
                          !e.row_sumsq && (d.N % 8 == 0) && (e.out_f32 || e.out_f16 || e.out_f16_relu);
   const bool inplace = e.res_f32 && e.res_f32 == e.out_f32;
   if (!plain_epi || inplace) return 0;
-  const int ref_pair_tiles = ((kSplitRefBatch * p.tiles_h * p.tiles_w + 1) / 2) * n_tiles;
-  if (ref_pair_tiles * 2 > max_pairs) return 0;
-  int s = max_pairs / ref_pair_tiles;
+  const int ref_tiles = kSplitRefBatch * p.tiles_h * p.tiles_w * n_tiles;
+  if (ref_tiles * 2 > max_ctas) return 0;
+  int s = max_ctas / ref_tiles;
   if (mode > 1) s = mode;
   if (s > p.k_iters / 4) s = p.k_iters / 4;
   if (s > 16) s = 16;
   // two or three segments only pay where the unsplit GEMM would leave through the register-direct epilogue (fp32 /
-  // residual / multi-output: measured 39 -> 30 us at 30x30); a plain fp16 output keeps its TMA-store epilogue (25 -> 28 us)
+  // residual / multi-output); a plain fp16 output keeps its TMA-store epilogue
   const bool tma_f16 = e.out_f16 && !e.out_f32 && !e.out_f16_relu && !e.res_f32 && !e.res2_f32;
   if (s < 4 && tma_f16 && mode <= 1) return 0;
   return s >= 2 ? s : 0;
@@ -260,33 +222,9 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     set_error("gemm: K=%d must be a multiple of %d", d.K, kGemmBK);
     return -1;
   }
-  int bn = (d.N > 128) ? 256 : 128;
-  {
-    // In-place fp32 residual GEMMs (attention proj, fc2): pick the tile width that minimises (waves x width) over the
-    // 74 CTA pairs. With N = 1024 and 29 row pairs, 256-wide tiles give 116 pair tiles = 1.57 -> 2 waves, 224-wide give
-    // 145 = 1.96 -> 2 waves of narrower tiles (-12 %). The per-element K order is unchanged, so results are identical.
-    static const int add_bn = getenv("LSEG_GEMM_ADD_BN") ? atoi(getenv("LSEG_GEMM_ADD_BN")) : 0;  // 0: automatic
-    const bool inplace_add = !d.conv && d.e.out_f32 && d.e.res_f32 == d.e.out_f32 && !d.e.res2_f32 && !d.e.res_f16 &&
-                             !d.e.out_f16 && !d.e.out_f16_relu && !d.e.out_row_sumsq && !d.e.relu_after_res &&
-                             d.e.store == STORE_ROWMAJOR &&
-                             (d.N % 8 == 0) && d.N >= 64 && (d.e.ldc % 4 == 0) && g_gemm_two_cta &&
-                             getenv("LSEG_GEMM_NO_TMA_STORE") == nullptr;  // == the EPI_TMA_ADD condition below
-    if (inplace_add && d.N > 128) {
-      if (add_bn == 128 || add_bn == 224 || add_bn == 256) {
-        bn = add_bn;
-      } else if (g_num_sms > 0) {
-        const long long m_pairs = ((d.M + kGemmBM - 1) / kGemmBM + 1) / 2;
-        const long long pairs = g_num_sms / 2;
-        auto cost = [&](int w) { return ((m_pairs * ((d.N + w - 1) / w) + pairs - 1) / pairs) * w; };
-        if (cost(224) < cost(256)) bn = 224;
-      }
-    }
-  }
-  plan->bn = bn;
-  plan->two_cta = g_gemm_two_cta;
   const int taps = d.conv ? d.kh * d.kw : 1;
   const long long ktot = static_cast<long long>(taps) * d.K;
-  if (d.w_rows < bn && d.w_rows < d.N) {
+  if (d.w_rows < kGemmBN && d.w_rows < d.N) {
     set_error("gemm: weight rows %d < N %d", d.w_rows, d.N);
     return -1;
   }
@@ -317,22 +255,20 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     const uint32_t box[2] = {kGemmBK, kGemmBM};
     if (make_tmap_f16(&p.tma_a, d.a, 2, dims, str, box)) return -1;
   }
-  p.num_n_tiles = (d.N + bn - 1) / bn;
+  p.num_n_tiles = (d.N + kGemmBN - 1) / kGemmBN;
   {
     const uint64_t dims[2] = {(uint64_t)ktot, (uint64_t)d.w_rows};
     const uint64_t str[1] = {(uint64_t)ktot * 2};
-    // CTA-pair kernel: each CTA of the pair loads half of the weight tile
-    const uint32_t box[2] = {kGemmBK, (uint32_t)(plan->two_cta ? bn / 2 : bn)};
+    const uint32_t box[2] = {kGemmBK, kGemmBN};
     if (make_tmap_f16(&p.tma_b, d.w, 2, dims, str, box)) return -1;
   }
-  // TMA-store epilogue: plain fp16 row-major outputs of the CTA-pair kernel (QKV, fc1, readout, 1x1 / 3x3
-  // convs feeding the next conv, head1, text in_proj / c_fc)
+  // TMA-store epilogue: plain fp16 row-major outputs (QKV, fc1, readout, 1x1 / 3x3 convs feeding the next conv,
+  // head1, text in_proj / c_fc)
   plan->epi = EPI_DIRECT;
-  plan->ew16 = 0;
   plan->ws_bytes = 0;
+  const int tiles = p.num_m_tiles * p.num_n_tiles;
   {
-    const int pair_tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    const int split = gemm_pick_split(d, p, p.num_n_tiles, g_num_sms / 2);
+    const int split = gemm_pick_split(d, p, p.num_n_tiles, g_num_sms);
     if (split) {
       plan->final_epi = d.e;
       p.split_fixed = split;
@@ -343,9 +279,8 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
       p.e.ldc = d.N;
       p.e.row_scale = 1.f;
       plan->ws_bytes = sizeof(float) * static_cast<size_t>(split) * d.M * d.N;
-      const int units = pair_tiles * split;
-      const int max_pairs = g_num_sms / 2;
-      plan->grid = 2 * (units < max_pairs ? units : max_pairs);
+      const int units = tiles * split;
+      plan->grid = units < g_num_sms ? units : g_num_sms;
       if (d.e.store == STORE_ROWMAJOR && (d.e.ldc % 8 != 0)) {
         set_error("gemm: ldc must be a multiple of 8");
         return -1;
@@ -356,8 +291,8 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
   {
     const GemmEpi& e = p.e;
     static const bool disabled = getenv("LSEG_GEMM_NO_TMA_STORE") != nullptr;
-    const bool rowmajor = plan->two_cta && !disabled && e.store == STORE_ROWMAJOR && (d.N % 8 == 0) && d.N >= 64;
-    if (e.relu_after_res && (e.store != STORE_ROWMAJOR || !e.res_f32 || e.res_f16 || e.out_row_sumsq || !plan->two_cta)) {
+    const bool rowmajor = !disabled && e.store == STORE_ROWMAJOR && (d.N % 8 == 0) && d.N >= 64;
+    if (e.relu_after_res && (e.store != STORE_ROWMAJOR || !e.res_f32 || e.res_f16 || e.out_row_sumsq)) {
       set_error("gemm: relu_after_res needs a row-major store and an fp32 residual");
       return -1;
     }
@@ -375,7 +310,6 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
         if (make_tmap_f16(&p.tma_c, e.out_f16, 2, dims, str, box)) return -1;
       }
       plan->epi = EPI_TMA_F16;
-      plan->ew16 = (bn == 256 && (p.k_iters <= 8 || e.act == ACT_GELU)) ? 1 : 0;
     } else if (rowmajor && !d.conv && e.out_f32 && e.res_f32 == e.out_f32 && !e.res2_f32 && !e.res_f16 &&
                !e.out_f16 && !e.out_f16_relu && !e.out_row_sumsq && !e.relu_after_res && (e.ldc % 4 == 0)) {
       // in-place fp32 residual stream: x += A W^T + b through a bulk tensor reduce-add (x is never read)
@@ -385,21 +319,12 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
       if (make_tmap(&p.tma_c, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, e.out_f32, 2, dims, str, box)) return -1;
       plan->epi = EPI_TMA_ADD;
       // stream-K style balancing when whole tiles would leave a ragged last wave
-      const int pair_tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-      const int max_pairs = g_num_sms / 2;
       static const int min_kit = getenv("LSEG_SPLITK_MIN_KITERS") ? atoi(getenv("LSEG_SPLITK_MIN_KITERS")) : 32;
       p.split_k =
-          (!g_deterministic && pair_tiles > max_pairs && pair_tiles % max_pairs != 0 && p.k_iters >= min_kit) ? 1 : 0;
+          (!g_deterministic && tiles > g_num_sms && tiles % g_num_sms != 0 && p.k_iters >= min_kit) ? 1 : 0;
     }
   }
-  if (plan->two_cta) {
-    const int pair_tiles = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    const int max_pairs = g_num_sms / 2;
-    plan->grid = 2 * (pair_tiles < max_pairs ? pair_tiles : max_pairs);
-  } else {
-    const int tiles = p.num_m_tiles * p.num_n_tiles;
-    plan->grid = tiles < g_num_sms ? tiles : g_num_sms;
-  }
+  plan->grid = tiles < g_num_sms ? tiles : g_num_sms;
   if (p.e.store == STORE_D2S && (p.e.d2s_cout % 32 != 0 || !p.e.out_f16)) {
     set_error("gemm: depth-to-space store needs cout %% 32 == 0 and an fp16 output");
     return -1;
@@ -430,49 +355,18 @@ static int gemm_run(const GemmPlan& plan, cudaStream_t stream) {
   return gemm_run_kernel(plan, stream);
 }
 static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream) {
-  {
-#define LSEG_LAUNCH_TC2(BN_, EPI_) \
-  launch_pdl(gemm_tc2_kernel<BN_, EPI_>, dim3(plan.grid), dim3(Gemm2Cfg<BN_, EPI_>::kThreads), Gemm2Cfg<BN_, EPI_>::kSmemBytes, stream, plan.p)
-    if (plan.bn == 256) {
-      if (plan.epi == EPI_TMA_F16 && plan.ew16)
-        launch_pdl(gemm_tc2_kernel<256, EPI_TMA_F16, 16>, dim3(plan.grid), dim3(Gemm2Cfg<256, EPI_TMA_F16, 16>::kThreads),
-                   Gemm2Cfg<256, EPI_TMA_F16, 16>::kSmemBytes, stream, plan.p);
-      else if (plan.epi == EPI_TMA_F16) LSEG_LAUNCH_TC2(256, EPI_TMA_F16);
-      else if (plan.epi == EPI_TMA_ADD) LSEG_LAUNCH_TC2(256, EPI_TMA_ADD);
-      else if (plan.p.split_fixed > 1)
-        launch_pdl(gemm_tc2_kernel<256, EPI_DIRECT, 8, true>, dim3(plan.grid), dim3(Gemm2Cfg<256, EPI_DIRECT>::kThreads),
-                   Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else if (plan.p.e.store == STORE_NCHW_T && plan.p.e.nchw_group > 0)
-        launch_pdl(gemm_tc2_kernel<256, EPI_DIRECT, 8, false, true>, dim3(plan.grid),
-                   dim3(Gemm2Cfg<256, EPI_DIRECT>::kThreads), Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else if (plan.p.e.relu_after_res)
-        launch_pdl(gemm_tc2_kernel<256, EPI_DIRECT, 8, false, false, true>, dim3(plan.grid),
-                   dim3(Gemm2Cfg<256, EPI_DIRECT>::kThreads), Gemm2Cfg<256, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else LSEG_LAUNCH_TC2(256, EPI_DIRECT);
-    } else if (plan.bn == 224) {
-      if (plan.epi != EPI_TMA_ADD) {
-        set_error("gemm: 224-wide tiles exist for the in-place residual epilogue only");
-        return -1;
-      }
-      LSEG_LAUNCH_TC2(224, EPI_TMA_ADD);
-    } else {
-      if (plan.epi == EPI_TMA_F16) LSEG_LAUNCH_TC2(128, EPI_TMA_F16);
-      else if (plan.epi == EPI_TMA_ADD) LSEG_LAUNCH_TC2(128, EPI_TMA_ADD);
-      else if (plan.p.split_fixed > 1)
-        launch_pdl(gemm_tc2_kernel<128, EPI_DIRECT, 8, true>, dim3(plan.grid), dim3(Gemm2Cfg<128, EPI_DIRECT>::kThreads),
-                   Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else if (plan.p.e.store == STORE_NCHW_T && plan.p.e.nchw_group > 0)
-        launch_pdl(gemm_tc2_kernel<128, EPI_DIRECT, 8, false, true>, dim3(plan.grid),
-                   dim3(Gemm2Cfg<128, EPI_DIRECT>::kThreads), Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else if (plan.p.e.relu_after_res)
-        launch_pdl(gemm_tc2_kernel<128, EPI_DIRECT, 8, false, false, true>, dim3(plan.grid),
-                   dim3(Gemm2Cfg<128, EPI_DIRECT>::kThreads), Gemm2Cfg<128, EPI_DIRECT>::kSmemBytes, stream, plan.p);
-      else LSEG_LAUNCH_TC2(128, EPI_DIRECT);
-    }
-#undef LSEG_LAUNCH_TC2
-    LSEG_CHECK_CUDA(cudaGetLastError());
-    return 0;
-  }
+#define LSEG_LAUNCH(KERNEL, EPI_) \
+  launch_pdl(KERNEL, dim3(plan.grid), dim3(GemmCfg<EPI_>::kThreads), GemmCfg<EPI_>::kSmemBytes, stream, plan.p)
+  if (plan.epi == EPI_TMA_F16) LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_F16>, EPI_TMA_F16);
+  else if (plan.epi == EPI_TMA_ADD) LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_ADD>, EPI_TMA_ADD);
+  else if (plan.p.split_fixed > 1) LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT);
+  else if (plan.p.e.store == STORE_NCHW_T && plan.p.e.nchw_group > 0)
+    LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT);
+  else if (plan.p.e.relu_after_res) LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT);
+  else LSEG_LAUNCH(gemm_tc_kernel<EPI_DIRECT>, EPI_DIRECT);
+#undef LSEG_LAUNCH
+  LSEG_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -491,7 +385,7 @@ static int mhsa_plan(const MhsaDesc& d, MhsaPlan* plan) {
   const uint64_t str[2] = {(uint64_t)3 * D * 2, (uint64_t)3 * D * d.N * 2};
   const uint32_t box[3] = {kMhsaDh, kMhsaTile, 1};
   if (make_tmap_f16(&p.tma_qkv, d.qkv, 3, dims, str, box)) return -1;
-  const uint32_t box64[3] = {kMhsaDh, kM2KT, 1};
+  const uint32_t box64[3] = {kMhsaDh, kMhsaKT, 1};
   if (make_tmap_f16(&p.tma_t64, d.qkv, 3, dims, str, box64)) return -1;
   p.out = d.out;
   p.n_tokens = d.N;
@@ -502,20 +396,15 @@ static int mhsa_plan(const MhsaDesc& d, MhsaPlan* plan) {
   plan->grid = dim3((d.N + kMhsaTile - 1) / kMhsaTile, d.B * d.heads, 1);
   return 0;
 }
-// variant: 0 mhsa2 (round-1 kernel: one polling MMA warp); 1 mhsa3 (one blocking MMA warp per stream, setmaxnreg);
-// 2 = 1 + packed-fp32 softmax arithmetic; 3 = 2 + one of four score pairs on the FMA-pipe exp2 polynomial; 4 = two of four;
-// 5..8 mhsa4 (P in tensor memory, TS-form PV MMA): 5 scalar arithmetic, 6 packed, 7 packed + 1/4 polynomial, 8 + 2/4.
+// variant (include/lseg_b200.h): the share of exponentials evaluated on the FMA pipe — 0, 1, 2, 5, 6: none; 3, 7: one
+// of four score pairs; 4, 8: two of four.
 static int mhsa_run_variant(const MhsaPlan& plan, int variant, cudaStream_t stream) {
   switch (variant) {
-    case 0: launch_pdl(mhsa2_kernel<0, false>, plan.grid, dim3(kM2Threads), kM2SmemBytes, stream, plan.p); break;
-    case 1: launch_pdl(mhsa3_kernel<false, 0>, plan.grid, dim3(kM3Threads), kM2SmemBytes, stream, plan.p); break;
-    case 2: launch_pdl(mhsa3_kernel<true, 0>, plan.grid, dim3(kM3Threads), kM2SmemBytes, stream, plan.p); break;
-    case 3: launch_pdl(mhsa3_kernel<true, 1>, plan.grid, dim3(kM3Threads), kM2SmemBytes, stream, plan.p); break;
-    case 4: launch_pdl(mhsa3_kernel<true, 2>, plan.grid, dim3(kM3Threads), kM2SmemBytes, stream, plan.p); break;
-    case 5: launch_pdl(mhsa4_kernel<false, 0>, plan.grid, dim3(kM3Threads), kM4SmemBytes, stream, plan.p); break;
-    case 6: launch_pdl(mhsa4_kernel<true, 0>, plan.grid, dim3(kM3Threads), kM4SmemBytes, stream, plan.p); break;
-    case 7: launch_pdl(mhsa4_kernel<true, 1>, plan.grid, dim3(kM3Threads), kM4SmemBytes, stream, plan.p); break;
-    case 8: launch_pdl(mhsa4_kernel<true, 2>, plan.grid, dim3(kM3Threads), kM4SmemBytes, stream, plan.p); break;
+    case 0: case 1: case 2: case 5: case 6:
+      launch_pdl(mhsa_kernel<0>, plan.grid, dim3(kMhsaThreads), kMhsaSmemBytes, stream, plan.p);
+      break;
+    case 3: case 7: launch_pdl(mhsa_kernel<1>, plan.grid, dim3(kMhsaThreads), kMhsaSmemBytes, stream, plan.p); break;
+    case 4: case 8: launch_pdl(mhsa_kernel<2>, plan.grid, dim3(kMhsaThreads), kMhsaSmemBytes, stream, plan.p); break;
     default: set_error("mhsa: unknown kernel variant %d", variant); return -1;
   }
   LSEG_CHECK_CUDA(cudaGetLastError());
@@ -836,7 +725,7 @@ int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int cau
   MhsaPlan plan;
   if (mhsa_plan(d, &plan)) return -1;
   plan.p.trace = trace;
-  mhsa2_kernel<kMhsaPolyDefault, true><<<plan.grid, kM2Threads, kM2SmemBytes, static_cast<cudaStream_t>(stream)>>>(plan.p);
+  mhsa_kernel<0, true><<<plan.grid, kMhsaThreads, kMhsaSmemBytes, static_cast<cudaStream_t>(stream)>>>(plan.p);
   LSEG_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -7,7 +7,7 @@
 //     attn = bmm(q, k^T) + mask              (fp32 accumulate, fp16 result)
 //     attn = softmax(attn, -1)               (fp32 arithmetic inside, NORMALISED result rounded to fp16)
 //     out  = bmm(attn, v)                    (fp32 accumulate, fp16 result)
-// which oracle/lseg_oracle.py:185-196 restates. The flash-style tensor-core kernel (mhsa2.cuh) keeps S in fp32 and
+// which oracle/lseg_oracle.py:185-196 restates. The flash-style tensor-core kernel (mhsa.cuh) keeps S in fp32 and
 // rounds the UN-normalised P, i.e. it has different rounding points; the text tower runs once per label set on K*77
 // tokens, so this kernel trades speed for those exact rounding points: plain CUDA cores, one CTA per (label, head),
 // one warp per query row, fp32 dot products in a fixed order. L <= 77 keys, head_dim 64.

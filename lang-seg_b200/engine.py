@@ -17,7 +17,7 @@ class Engine:
     def __init__(self, state_dict, device, arch_option=0, block_depth=0, activation="lrelu", backbone="clip_vitl16_384"):
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("lseg_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("lseg_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
         self.device = device
         self.lib = _lib.load()
         with torch.cuda.device(device):

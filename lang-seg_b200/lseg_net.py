@@ -1,4 +1,4 @@
-"""Drop-in `LSegNet` / `LSegNetZS` whose forward runs on the sm_100a engine.
+"""Drop-in `LSegNet` / `LSegNetZS` whose forward runs on the sm_90a engine.
 
 Mirrors the reference interface for the hot path (SURVEY.md section 8(b)):
   * constructor signatures of modules/models/lseg_net.py:208-226 and lseg_net_zs.py:219-239;
@@ -298,7 +298,7 @@ class _LSegBase(nn.Module):
         from .engine import Engine
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("lseg_b200.LSegNet runs on CUDA (B200, sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("lseg_b200.LSegNet runs on CUDA (H100, sm_90a) only; there is no CPU fallback")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
         shared = self._shared
@@ -332,7 +332,7 @@ class _LSegBase(nn.Module):
 
 
 class LSegNet(_LSegBase):
-    """Network for semantic segmentation — B200-native forward (reference: lseg_net.py:208-226)."""
+    """Network for semantic segmentation — H100-native forward (reference: lseg_net.py:208-226)."""
 
     def __init__(self, labels, path=None, scale_factor=0.5, crop_size=480, **kwargs):
         super().__init__()

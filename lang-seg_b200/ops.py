@@ -152,7 +152,7 @@ def set_deterministic(on):
 
 
 def mhsa_trace(qkv, B, N, heads, causal=False):
-    """Debug: (out, trace[16 CTAs, 10 warps, 256]) with clock64 << 8 | tag stamps (tools/mhsa_trace.py)."""
+    """Debug: (out, trace[16 CTAs, 10 warps, 256]) with clock64 << 8 | tag stamps."""
     out = torch.empty((B * N, heads * 64), dtype=torch.float16, device=qkv.device)
     trace = torch.zeros((16, 10, 256), dtype=torch.int64, device=qkv.device)
     check(load().lseg_mhsa_trace(_ptr(qkv, torch.float16), _ptr(out), B, N, heads, int(causal), _ptr(trace), _stream()))

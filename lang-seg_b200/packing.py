@@ -1,10 +1,10 @@
-"""State-dict -> packed device buffers for the sm_100a engine (host-side, one-off per weight load).
+"""State-dict -> packed device buffers for the sm_90a engine (host-side, one-off per weight load).
 
 Input: the reference's state dict (key names of SURVEY.md Appendix C, fp32). Output: the
 `lseg_weights` descriptor of include/lseg_b200.h plus the tensors that back its pointers.
 
 Layouts
-  * every GEMM weight is fp16 [N, K] row-major (K contiguous = "K-major" UMMA operand), rows padded
+  * every GEMM weight is fp16 [N, K] row-major (K contiguous = "K-major" wgmma operand), rows padded
     with zeros to a multiple of 128 so a TMA box never exceeds the tensor;
   * 3x3 convs are tap-major: [N, (ky, kx, c)]  (the implicit-GEMM K loop walks taps, then channels);
   * ConvTranspose2d with kernel == stride becomes a GEMM with N = (i, j, co) and a depth-to-space

@@ -3,7 +3,7 @@
 The image path has no cross-image operation in eval mode (BatchNorm uses running statistics), so the
 batch shards across ranks with NO data-path collective; weights are resident per rank and text features
 are computed redundantly per rank (150 KB, cheaper than a broadcast). The only exchange is the gather of
-the final logits: an NCCL all-gather over NVLink 5 / NVSwitch on B200 (gloo in the CPU tests).
+the final logits: an NCCL all-gather over NVLink / NVSwitch (gloo in the CPU tests).
 This replaces the reference's single-process, thread-per-GPU DataParallel with a per-call parameter
 broadcast (additional_utils/models.py:35-53,183-248).
 """
@@ -301,8 +301,8 @@ class LogitsGather:
         if not self.materialize:
             return
         lib = _lib.load()
-        # background=True: the shared-memory-free kernel meant to run beside the next step's trunk (measured: it does
-        # not — see DESIGN.md section 6 — so the default is the faster shared-memory kernel)
+        # background=True: the shared-memory-free kernel meant to run beside the next step's trunk; the default is the
+        # shared-memory kernel (same values bit for bit)
         fn = lib.lseg_upsample2x_nchw_bg if self.background else lib.lseg_upsample2x_nchw
         per = max(1, 65535 // (self.B * self.K))  # images per launch (grid.y limit)
         cs = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)

@@ -1,13 +1,13 @@
 """TEST INFRASTRUCTURE — generate the golden fixtures under tests/golden/ from the REAL reference.
 
-Runs ONLY in the build container (needs /root/reference): imports the reference's
+Needs a lang-seg checkout named by LSEG_REFERENCE_ROOT: imports the reference's
 modules/models/lseg_net.py unchanged through oracle/ref_standins.py, loads the seeded synthetic state
 dict (oracle/synth.py), runs LSegNet.forward on seeded inputs, verifies that the oracle restatement
 (oracle/lseg_oracle.py) reproduces it, and writes small fixtures:
 
   tests/golden/ref_small.npz    B=2, 64x96, K=5   : full logits (fp16-exact values stored as fp32), taps/path
                                                     checksums
-  tests/golden/ref_480_k150.npz B=1, 480x480, K=150: logits at a stride-8 pixel lattice, full argmax mask
+  tests/golden/ref_480_k150.npz B=1, 480x480, K=150: logits at a stride-24 pixel lattice, full argmax mask
                                                     (uint8), text features, per-stage statistics
   tests/golden/ref_480_k2.npz   B=1, 480x480, ['cat','other'] (BASELINE.json configs[0])
   tests/golden/ref_zs.npz       zero-shot path (lseg_net_zs.py) B=3, 96x96, PASCAL label file
@@ -31,6 +31,7 @@ from oracle import ref_standins as R  # noqa: E402
 from oracle import synth  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
+LATTICE = {"k150": 24, "k2": 8}  # pixel stride of the stored logits: keeps each fixture < 1 MB
 
 
 def _stats(t):
@@ -97,7 +98,7 @@ def main():
             tf = tf / tf.norm(dim=-1, keepdim=True)
         top2 = ref.topk(2, dim=1).values
         np.savez_compressed(os.path.join(GOLD, f"ref_480_{tag}.npz"),
-                            logits_lattice=ref[:, :, ::8, ::8].numpy(),
+                            logits_lattice=ref[:, :, ::LATTICE[tag], ::LATTICE[tag]].numpy(),
                             argmax=ref.argmax(1).to(torch.uint8).numpy(),
                             margin_f16=(top2[:, 0] - top2[:, 1]).half().numpy(),
                             text_features=tf.numpy(),
@@ -129,6 +130,11 @@ def main():
     got = O.lseg_forward_zs(x, class_info, texts, sd)
     _check("zero-shot logits", ref, got, 3e-3)
     np.savez_compressed(os.path.join(GOLD, "ref_zs.npz"), logits=ref.numpy(), class_info=class_info.numpy())
+    # the reference LSegNet built by its own constructor (ref_standins.build_reference_net), 3 labels, 64x64
+    labels3 = ["cat", "other", "tree"]
+    with torch.no_grad():
+        ref = R.build_reference_net(sd, labels3)(synth.make_image(1, 64, 64, seed=9))
+    np.savez_compressed(os.path.join(GOLD, "ref_net_small.npz"), logits=ref.numpy())
     print("golden fixtures written to", GOLD)
 
 

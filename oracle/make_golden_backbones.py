@@ -72,7 +72,7 @@ def make(TAG, BACKBONE):
             out["small_logits"] = ref.numpy()
             out["small_labels"] = np.array(labels)
         else:
-            out["k150_logits_lattice"] = ref[:, :, ::8, ::8].numpy()
+            out["k150_logits_lattice"] = ref[:, :, ::24, ::24].numpy()  # keeps the fixture < 1 MB
             out["k150_argmax"] = ref.argmax(1).to(torch.uint8).numpy()
             out["k150_margin_f16"] = (top2[:, 0] - top2[:, 1]).half().numpy()
         out[f"{tag}_floor"] = np.array(e2)  # the reference's two executions of its fp16 text tower, in the logits

@@ -6,7 +6,7 @@ small, exactly batch-invariant stand-in network (elementwise arithmetic only), a
 and outputs in tests/golden/ref_multiscale.npz. tests/test_evaluator_cpu.py replays them through
 lseg_b200.evaluator.MultiScaleEvaluator.
 
-    python oracle/make_golden_eval.py        # needs /root/reference (this container only)
+    LSEG_REFERENCE_ROOT=<lang-seg checkout> python oracle/make_golden_eval.py
 """
 import contextlib
 import io
@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("LSEG_REFERENCE_ROOT", "")
 
 
 class StandInNet(nn.Module):

@@ -85,7 +85,7 @@ def main():
         if tag == "small":
             out["small_logits"] = ref.numpy()
         else:
-            out["s480_logits_lattice"] = ref[:, :, ::4, ::4].numpy()
+            out["s480_logits_lattice"] = ref[:, :, ::8, ::8].numpy()  # keeps the fixture < 1 MB
             out["s480_argmax"] = ref.argmax(1).to(torch.uint8).numpy()
             top2 = ref.topk(2, dim=1).values
             out["s480_margin_f16"] = (top2[:, 0] - top2[:, 1]).half().numpy()

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE — stand-ins that let /root/reference's own modules import and run unchanged.
+"""TEST INFRASTRUCTURE — stand-ins that let the reference checkout's own modules import and run unchanged.
 
 The reference depends on third-party packages that are not installed here (timm 0.4.12, OpenAI clip
 @04f4dc2, PyTorch-Encoding, pytorch_lightning, matplotlib; SURVEY.md Appendix B). This module registers
@@ -9,9 +9,8 @@ The reference depends on third-party packages that are not installed here (timm 
     fp32-computing LayerNorm), weights converted to fp16 like clip.load(device='cuda') does;
     `clip.tokenize` -> oracle.synth.tokenize (no BPE vocabulary offline);
   * inert stubs for encoding / pytorch_lightning / matplotlib so modules/lseg_module.py imports.
-Used by make_golden.py, by the tests that drive the unmodified reference (they skip when neither /root/reference nor
-the baseline/_ref copy made by oracle/make_ref.sh is present) and by bench.py --impl reference; nothing here is
-imported by the product path.
+Used by the golden-fixture generators (oracle/make_golden*.py); nothing here is imported by the product path, the
+tests or bench.py.
 """
 import os
 import sys
@@ -22,21 +21,15 @@ import torch
 import torch.nn as nn
 
 def _find_reference_root():
-    """/root/reference in the build container; on the GPU box the byte-for-byte copy oracle/make_ref.sh installs under
-    baseline/_ref/ (git-ignored, travels with the gpurun snapshot)."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    for cand in (os.environ.get("LSEG_REFERENCE_ROOT"), "/root/reference",
-                 os.path.join(os.path.dirname(here), "baseline", "_ref")):
-        if cand and os.path.isdir(os.path.join(cand, "modules", "models")):
-            return cand
-    return "/root/reference"
+    """The lang-seg checkout named by $LSEG_REFERENCE_ROOT. Only the golden-fixture generators need it."""
+    return os.environ.get("LSEG_REFERENCE_ROOT", "")
 
 
 REFERENCE_ROOT = _find_reference_root()
 
 
 def reference_available():
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "modules", "models"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "modules", "models"))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -224,9 +217,9 @@ def _clip_load(name, device="cpu", jit=False):
 
 
 def install(with_lightning_stack=True):
-    """Register the stand-ins and put /root/reference on sys.path. Idempotent."""
+    """Register the stand-ins and put the reference checkout on sys.path. Idempotent."""
     if not reference_available():
-        raise FileNotFoundError(f"{REFERENCE_ROOT} is not available (run oracle/make_ref.sh in the build container)")
+        raise FileNotFoundError(f"{REFERENCE_ROOT} is not a lang-seg checkout (set LSEG_REFERENCE_ROOT)")
     here = os.path.dirname(os.path.abspath(__file__))
     sys.path.insert(0, os.path.dirname(here))
     from oracle import synth
@@ -314,7 +307,7 @@ def build_reference_module(state_dict=None, drop_in=False, **overrides):
     drop_in=False: with the reference's own `LSegNet` (modules/models/lseg_net.py) — the CPU baseline.
     drop_in=True : the one-line import swap of INTEGRATION.md applied WITHOUT editing the file: the module name
                    `modules.models.lseg_net` is pre-bound to a shim whose `LSegNet` is lseg_b200's, so
-                   `from .models.lseg_net import LSegNet` (modules/lseg_module.py:8) resolves to the B200 drop-in.
+                   `from .models.lseg_net import LSegNet` (modules/lseg_module.py:8) resolves to the H100 drop-in.
     The label file is opened relative to the cwd (modules/lseg_module.py:99), hence the chdir."""
     install()
     for name in ("modules.lseg_module", "modules.lsegmentation_module", "modules.models.lseg_net"):

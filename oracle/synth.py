@@ -4,7 +4,7 @@ No checkpoints, CLIP BPE vocabulary or datasets exist offline (SURVEY.md Appendi
 parity/bench run uses this deterministic stand-in data. Weights come from numpy's PCG64 stream
 (bit-reproducible across machines for the same numpy version), with the state-dict key names and
 shapes of SURVEY.md Appendix C so the same dict loads into the reference modules, the oracle and
-the B200 build. Init scales mirror the constructors (timm trunc_normal .02, torch Conv2d default
+the H100 build. Init scales mirror the constructors (timm trunc_normal .02, torch Conv2d default
 kaiming-uniform, CLIP initialize_parameters); LayerNorm/BatchNorm statistics and biases are
 perturbed so that folding and bias paths are actually exercised.
 """

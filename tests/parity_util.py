@@ -25,10 +25,16 @@ def state_dict(seed=0, backbone="clip_vitl16_384"):
 
 
 def rel_err(got, ref):
-    """max |got-ref| / max |ref| (the '1e-3 relative' metric of BASELINE.md section 3)."""
+    """max |got-ref| / max |ref| (the '1e-3 relative' metric of BASELINE.json's north_star)."""
     got = got.detach().float().cpu()
     ref = ref.detach().float().cpu()
     return ((got - ref).abs().max() / (ref.abs().max() + 1e-12)).item()
+
+
+def on_lattice(t, lat):
+    """t [B, K, H, W] sampled on the regular pixel lattice a golden fixture stores (lat [B, K, H / s, W / s])."""
+    s = t.shape[-1] // lat.shape[-1]
+    return t[:, :, ::s, ::s]
 
 
 def rms_rel_err(got, ref):

@@ -282,7 +282,8 @@ MHSA_SHAPES = [
     (1, 1937, 4, False, 1.0), (1, 2117, 3, False, 1.0), (1, 2117, 1, False, 3.0)]
 
 
-# variant None = the kernel the engine runs; 0 = round-1 kernel, 1..4 = mhsa3, 5..8 = mhsa4 (include/lseg_b200.h)
+# variant None = the kernel the engine runs; 0..8 = every number lseg_mhsa_variant accepts: 0/1/2/5/6 all exponentials
+# on the MUFU pipe, 3/7 one of four score pairs on the FMA pipe, 4/8 two of four (include/lseg_b200.h)
 @pytest.mark.parametrize("variant", [None, 0, 1, 2, 3, 4, 5, 6, 7, 8])
 @pytest.mark.parametrize("B,N,heads,causal,amp", MHSA_SHAPES)
 def test_mhsa(ops, B, N, heads, causal, amp, variant):

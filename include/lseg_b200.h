@@ -101,7 +101,9 @@ int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* st
  * partial sums are reduce-added in arrival order (differences at the fp32 rounding level, hence off by default). */
 int lseg_set_deterministic(int on);
 /* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTAs
- * into trace ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). */
+ * into trace ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). Row w of a CTA is
+ * warp w: rows 4-7 are consumer warpgroup 0 and rows 8-11 warpgroup 1, each stamping only the tiles it owns (every
+ * other entry of the CTA's work list); the other rows stay zero. Stamp = clock64() << 8 | tag. */
 int lseg_debug_gemm_trace(unsigned long long* trace);
 /* Debug: same computation, additionally stamps clock64() at the pipeline hand-off points of 16 sampled CTAs into
  * trace ([16][10 warps][256] uint64 device memory, zero-initialised by the caller). */

@@ -172,6 +172,23 @@ __device__ __forceinline__ bool elect_one_sync() {
 }
 __device__ __forceinline__ int warp_idx_sync() { return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0); }
 
+// Per-warpgroup register budget (all 128 threads of the warpgroup execute it): a warpgroup that only issues TMA hands
+// registers back to the pool, and the MMA warpgroups claim them. The budgets of all warpgroups must fit the CTA's
+// allocation at launch (registers per thread from ptxas x threads).
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// Named barriers (ids 1..15; 0 is __syncthreads). `threads` counts every thread that syncs or arrives, a multiple of 32:
+// bar_arrive signals without waiting, so a pair of warpgroups can hand a turn from one to the other.
+__device__ __forceinline__ void bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 
 // ---- proxies / fences --------------------------------------------------------------------
 // generic-proxy smem writes -> visible to the async proxy (TMA stores / wgmma operand reads)

@@ -7,12 +7,19 @@
 // and 3x3 stride-1 convs as implicit GEMM (the A tile of tap (dy,dx) is a shifted 4-D TMA box of
 // the NHWC activation; TMA zero-fills the padding halo).
 //
-// Roles (one CTA per SM, persistent over a static round-robin list of 128 x 128 tiles):
-//   warpgroup 0   TMA producer (warp 0, one elected lane): fills the A/B smem ring (128B-swizzled, K-major)
-//   warpgroups 1-2  consumers: each issues wgmma m64n128k16 for 64 of the tile's 128 rows (accumulator in registers),
-//                 then stages its fp32 accumulators in shared memory, and the 8 consumer warps run the epilogue with
-//                 thread <-> output row (warp = 32 rows x 64 columns): scale/bias/act/residual -> global.
-// The producer runs up to kStages k-chunks ahead, so the next tile's operands stream in during the epilogue.
+// Roles (one CTA per SM, persistent over a static round-robin list of 128 x 128 tiles), "ping-pong" schedule:
+//   warpgroup 0   TMA producer (warp 0, one elected lane; 24 registers): fills the A/B smem ring (128B-swizzled,
+//                 K-major) in list order
+//   warpgroups 1-2  consumers (240 registers): the list's entries alternate between them. A warpgroup computes its whole
+//                 tile (two wgmma m64n128k16 per k16 step, 2 x 64 fp32 accumulators per thread), then stages it in its
+//                 own shared-memory area one 64-column half at a time, and its 4 warps run the epilogue with thread <->
+//                 output row (warp = 32 rows x 64 columns per half): scale/bias/act/residual -> global.
+// The MMA turn passes from one warpgroup to the other in list order (named barriers), so one warpgroup's epilogue
+// runs while the other's MMAs keep the tensor cores busy; the tensor pipe idles only where an epilogue takes longer
+// than a main loop, or where a CTA owns a single tile. The accumulation order of every output element (the same
+// k16 chunks through the same m64n128k16 instruction) does not depend on which warpgroup computes the tile.
+// Measured (B=8, 480x480, H100 80GB HBM3 SXM at a 700 W power limit, tools/gemm_shapes.py): ViT linears 460-530
+// TFLOP/s (QKV, fc1) and 320-410 (proj, fc2); 3x3 decoder convs 310-440 at 60^2 / 120^2.
 //
 // Epilogue modes:
 //   EPI_DIRECT   stores straight from registers, thread <-> accumulator row.
@@ -78,7 +85,8 @@ struct GemmParams {
   int split_fixed;       // EPI_DIRECT, >= 2: every tile's K loop is cut into this many equal segments, each a work unit of
   long long split_rows;  //   its own; segment s stores its RAW fp32 partial at row (s * split_rows + row) of out_f32 and
                          //   splitk_reduce_kernel sums the segments in index order (deterministic) and applies the epilogue
-  unsigned long long* trace;  // debug timeline ([2 CTAs][20 warps][512] of clock64 << 8 | tag), normally nullptr
+  unsigned long long* trace;  // debug timeline ([2 CTAs][20 warps][512] of clock64 << 8 | tag; rows 4-11 = consumer
+                              // warps, layout in lseg_debug_gemm_trace), normally nullptr
   int probe;  // measurement only (results are garbage when non-zero):
               //   1 = skip epilogue work, 2 = skip TMA loads, 4 = skip MMA issue
   GemmEpi e;
@@ -338,13 +346,17 @@ __device__ __forceinline__ bool gemm_row_map(const GemmParams& p, int m_tile, in
   return (m_tile < p.num_m_tiles) && (grow < p.M);
 }
 
-constexpr int kEpiStageBytes = 2 * 4096;  // per epilogue warp: two 32-row x 128 B swizzled tiles (TMA epilogues)
+// Staged accumulators: one warpgroup's 128 rows x 64 fp32 columns (a column half of its tile), rows of 256 B with no
+// padding; the 16-byte chunk q of row r sits at chunk q ^ (r & 7), so the 8 rows a quarter-warp reads (thread <-> row)
+// and the 4 rows a fragment store touches spread over the banks.
+constexpr int kAccCols = kGemmBN / 2;
+__device__ __forceinline__ int gemm_acc_chunk(int q, int r) { return q ^ (r & 7); }
 
-// 32 consecutive fp32 accumulators of one row of the staged tile (16-byte aligned)
-__device__ __forceinline__ void gemm_acc_ld32(const float* src, uint32_t (&v)[32]) {
+// fp32 accumulators [32 c, 32 c + 32) of staged row r (acc_row = the row's start)
+__device__ __forceinline__ void gemm_acc_ld32(const float* acc_row, int c, int r, uint32_t (&v)[32]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float4 q = reinterpret_cast<const float4*>(src)[i];
+    const float4 q = reinterpret_cast<const float4*>(acc_row)[gemm_acc_chunk(8 * c + i, r)];
     v[4 * i] = __float_as_uint(q.x);
     v[4 * i + 1] = __float_as_uint(q.y);
     v[4 * i + 2] = __float_as_uint(q.z);
@@ -353,7 +365,7 @@ __device__ __forceinline__ void gemm_acc_ld32(const float* src, uint32_t (&v)[32
 }
 
 // Epilogue of one 128 x (ncols) accumulator slab for one warp (r = quarter*32 + lane = this thread's row); acc_row is
-// this thread's row of the fp32 accumulator tile staged in shared memory, at the warp's first column.
+// this thread's row of the staged accumulators (gemm_acc_ld32), whose column 0 is output column n_base.
 // SINGLE_BUF: one 4 KB staging tile per warp instead of two (leaves the shared memory to the accumulator tile and the
 // operand ring; the warp then waits for its previous bulk store to finish reading before it refills the buffer).
 template <int EPI, bool SINGLE_BUF = false, bool GROUPED = false, bool RELU_RES = false, typename WaitFn>
@@ -405,7 +417,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
       }
       uint32_t v[32];
       __syncwarp();
-      gemm_acc_ld32(acc_row + c * 32, v);
+      gemm_acc_ld32(acc_row, c, r, v);
       float f[32];
       gemm_epilogue_math(e, p.N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
       if (valid) {
@@ -441,7 +453,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
       if (n0 >= p.N) break;  // warp-uniform
       uint32_t v[32];
       __syncwarp();
-      gemm_acc_ld32(acc_row + c * 32, v);
+      gemm_acc_ld32(acc_row, c, r, v);
       tr(2);
       float f[32];
       gemm_epilogue_math(e, p.N, v, grow_c, n0, bias_off, valid, f, cc, c, first_k);
@@ -507,7 +519,9 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
 // ==========================================================================================
 // The kernel: persistent CTAs over 128 x 128 output tiles (warp roles in the header comment).
 //   full barrier  : per stage, armed by the producer with the stage's byte count; the TMA loads credit it
-//   empty barrier : per stage, one arrival per consumer warp once its warpgroup's MMAs have read the stage
+//   empty barrier : per stage, one arrival per warp of the consumer warpgroup whose MMAs have read the stage
+//   named barriers 1 / 2 : the MMA turn of consumer warpgroup 0 / 1 (ping-pong order, see the kernel)
+//   named barriers 3 / 4 : consumer warpgroup 0 / 1 alone (its accumulator staging area)
 // ==========================================================================================
 template <int EPI>
 struct GemmCfg {
@@ -518,14 +532,35 @@ struct GemmCfg {
   static constexpr int kThreads = 128 + 32 * kEpiWarps;   // + the producer warpgroup
   static constexpr int kEpiBufBytes = 4096;               // one 32-row x 128 B TMA-store staging tile per warp
   static constexpr int kStageOutBytes = (EPI == EPI_DIRECT) ? 0 : kEpiWarps * kEpiBufBytes;
-  static constexpr int kAccStride = kGemmBN + 4;          // fp32 row stride of the staged accumulators (bank spread)
-  static constexpr int kAccBytes = kGemmBM * kAccStride * 4;
-  // operand ring | per-warp TMA-store staging (1024 B aligned) | accumulator tile | mbarriers: <= 227 KB
-  static constexpr int kStages = (EPI == EPI_DIRECT) ? 4 : 3;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + kAccBytes + 1024 + 256;
+  static constexpr int kAccBytes = kGemmBM * kAccCols * 4;  // per consumer warpgroup: one staged column half
+  // operand ring | per-warp TMA-store staging (1024 B aligned) | 2 accumulator staging areas | mbarriers: <= 227 KB
+  static constexpr int kStages = (EPI == EPI_DIRECT) ? 5 : 4;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + 2 * kAccBytes + 1024 + 256;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory per CTA");
+  // 128 x 24 + 256 x 240 <= 65536 (= 384 x 168 at launch): what the producer warpgroup gives back, the consumers take
+  // (two 64 x 128 fp32 accumulators are 128 registers per consumer thread)
+  static constexpr int kProducerRegs = 24;
+  static constexpr int kConsumerRegs = 240;
 };
 
-__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// Fragment -> staging for column half H of the 64 tile rows whose staged row 0 is acc_half; acc holds them as wgmma lays
+// them out (warp wl: rows 16 wl + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)). The staged registers are zeroed
+// afterwards: the next tile's first MMA ignores the accumulator (scale-d = 0), so they are dead values instead of
+// registers held across the epilogue.
+template <int H>
+__device__ __forceinline__ void gemm_stage_half(float* acc_half, float (&acc)[64], int wl, int lane) {
+  const int r = wl * 16 + (lane >> 2);
+  float* d0 = acc_half + r * kAccCols + 2 * (lane & 1);
+  float* d1 = d0 + 8 * kAccCols;  // row r + 8: same swizzle as row r
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    const int j = 8 * H + jj;
+    const int q = gemm_acc_chunk(2 * jj + ((lane & 3) >> 1), r);
+    *reinterpret_cast<float2*>(d0 + 4 * q) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(d1 + 4 * q) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    acc[4 * j] = acc[4 * j + 1] = acc[4 * j + 2] = acc[4 * j + 3] = 0.f;
+  }
+}
 
 // FIXED_SPLIT: the deterministic split-K schedule (GemmParams::split_fixed) is its own instantiation, so its index
 // arithmetic stays out of the other kernels.
@@ -538,8 +573,8 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_out = smem + Cfg::kStages * Cfg::kStageBytes;
-  float* acc_tile = reinterpret_cast<float*>(stage_out + Cfg::kStageOutBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_tile) + Cfg::kAccBytes);
+  float* acc_stage = reinterpret_cast<float*>(stage_out + Cfg::kStageOutBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_stage) + 2 * Cfg::kAccBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
 
@@ -554,7 +589,7 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     if (EPI != EPI_DIRECT) tma_prefetch_desc(&p.tma_c);
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], Cfg::kEpiWarps);
+      mbar_init(&empty_bar[i], 4);
     }
     mbar_fence_init();
   }
@@ -616,9 +651,11 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     return sc;
   };
 
-  if (warp == 0) {
-    // ===================== TMA producer (converged warp, elected issuing lane) =====================
-    const bool leader = elect_one_sync();
+  if (warp < 4) {
+    // ===================== TMA producer warpgroup: warp 0 issues, warps 1-3 only hand their registers back =====================
+    setmaxnreg_dec<Cfg::kProducerRegs>();
+    if (warp != 0) return;
+    const bool leader = elect_one_sync();  // converged warp, elected issuing lane
     int stage = 0;
     uint32_t phase = 0;
     Sched sc = make_sched();
@@ -635,7 +672,8 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
         cw0 = (t % p.tiles_w) * kConvTW;
       }
       for (int kit = k_begin; kit < k_end; ++kit) {
-        mbar_wait(&empty_bar[stage], phase ^ 1, 21);
+        // inlined wait: an out-of-line callee cannot be shared by warpgroups with different setmaxnreg budgets
+        mbar_wait_inl(&empty_bar[stage], phase ^ 1, 21);
         uint8_t* sa = smem + stage * Cfg::kStageBytes;
         uint8_t* sb = sa + Cfg::kABytes;
         if (p.probe & 2) {
@@ -665,43 +703,61 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
-    // ===================== consumers: MMA main loop, then the epilogue =====================
-    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of the tile in the main loop
-    const int wl = warp & 3;         // warp within its warpgroup: accumulator rows 16 wl .. 16 wl + 15
-    const int ew = warp - 4;
-    const int quarter = ew & 3;      // epilogue: rows [32 quarter, +32), columns [64 half, +64)
-    const int half = ew >> 2;
-    const int r = quarter * 32 + lane;
-    const int col0 = half * 64;
-    const float* acc_row = acc_tile + r * Cfg::kAccStride + col0;
-    uint8_t* stage_buf = stage_out + ew * Cfg::kEpiBufBytes;
+  } else {
+    // ===================== consumers: ping-pong over the CTA's work list =====================
+    // Entry i of the list belongs to warpgroup i % 2, which runs the main loop of the whole 128 x 128 tile (two
+    // m64n128k16 per k16 step: rows 0-63 and 64-127) and then its epilogue. The producer fills the ring in list order,
+    // so the warpgroups take their MMA turns in list order: warpgroup w waits for its turn (barrier 1 + w) before its
+    // first full-barrier wait (the parity of a ring stage names one fill only once the previous entry has consumed its
+    // chunks) and hands the turn on as soon as its MMAs are issued. Its epilogue then runs during the other
+    // warpgroup's main loop.
+    setmaxnreg_inc<Cfg::kConsumerRegs>();
+    const int wg = (warp - 4) >> 2;
+    const int wl = warp & 3;       // warp within its warpgroup: main loop fragment rows 16 wl .. 16 wl + 15 of each
+    const int r = wl * 32 + lane;  // 64-row half; epilogue tile row r (thread <-> row)
+    float* acc_half = acc_stage + wg * (Cfg::kAccBytes / 4);
+    const float* acc_row = acc_half + r * kAccCols;
+    uint8_t* stage_buf = stage_out + (warp - 4) * Cfg::kEpiBufBytes;
     int store_groups = 0;
     int stage = 0;
     uint32_t phase = 0;
     GemmTrace tr;
     if (p.trace && lane == 0 && (cta == 0 || cta == num_ctas / 2)) tr.w = p.trace + ((cta == 0 ? 0 : 1) * 20 + warp) * 512;
     tr(0);
-    float acc[64];
+    float acc0[64], acc1[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
     Sched sc = make_sched();
     int tile, k_begin, k_end;
-    while (sc.next(tile, k_begin, k_end)) {
+    bool more = sc.next(tile, k_begin, k_end);
+    for (int idx = 0; more; ++idx) {
       const int m_tile = tile % p.num_m_tiles;
       const int n_tile = tile / p.num_m_tiles;
+      const int kb = k_begin, ke = k_end;
+      const int seg = FIXED_SPLIT ? sc.seg : 0;
+      more = sc.next(tile, k_begin, k_end);  // entry idx + 1
+      if ((idx & 1) != wg) {  // the other warpgroup's entry: step over its ring fills
+        const int s = stage + (ke - kb);
+        phase ^= (s / Cfg::kStages) & 1;
+        stage = s % Cfg::kStages;
+        continue;
+      }
+      if (idx > 0) bar_sync(1 + wg, 256);
       int prev = -1;
-      for (int kit = k_begin; kit < k_end; ++kit) {
-        mbar_wait(&full_bar[stage], phase, 23);
+      for (int kit = kb; kit < ke; ++kit) {
+        mbar_wait_inl(&full_bar[stage], phase, 23);
         __syncwarp();
-        const uint32_t a_base = smem_u32(smem + stage * Cfg::kStageBytes) + wg * (64 * 128);
-        const uint32_t b_base = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
+        const uint32_t a_base = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint32_t b_base = a_base + Cfg::kABytes;
         if (!(p.probe & 4)) {
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kGemmBK / 16; ++k)
-            wgmma_m64n128k16_ss(acc, wgmma_desc_sw128(a_base + k * 32, 1024, 16),
-                                wgmma_desc_sw128(b_base + k * 32, 1024, 16), (kit != k_begin) || (k != 0));
+          for (int k = 0; k < kGemmBK / 16; ++k) {
+            const uint64_t db = wgmma_desc_sw128(b_base + k * 32, 1024, 16);
+            const uint32_t accumulate = (kit != kb) || (k != 0);
+            wgmma_m64n128k16_ss(acc0, wgmma_desc_sw128(a_base + k * 32, 1024, 16), db, accumulate);
+            wgmma_m64n128k16_ss(acc1, wgmma_desc_sw128(a_base + 64 * 128 + k * 32, 1024, 16), db, accumulate);
+          }
           wgmma_commit();
         }
         wgmma_wait<1>();  // the previous chunk's MMAs have read their stage: hand it back to the producer
@@ -709,30 +765,27 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
         prev = stage;
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
+      if (more) bar_arrive(1 + (wg ^ 1), 256);  // entry idx + 1 is the other warpgroup's
       wgmma_wait<0>();
-      wgmma_reg_fence(acc);
+      wgmma_reg_fence(acc0);
+      wgmma_reg_fence(acc1);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       tr(12);
-      // stage the accumulators (fragment rows 64 wg + 16 wl + lane/4 (+8), columns 8 j + 2 (lane % 4) (+1)) once the
-      // previous tile's epilogue has read the tile
-      consumer_bar_sync();
-      {
-        float* d0 = acc_tile + (wg * 64 + wl * 16 + (lane >> 2)) * Cfg::kAccStride + 2 * (lane & 3);
-        float* d1 = d0 + 8 * Cfg::kAccStride;
-#pragma unroll
-        for (int j = 0; j < kGemmBN / 8; ++j) {
-          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(d1 + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      // the next tile's first MMA ignores the accumulator (scale-d = 0): dead values, not 64 registers held across the
-      // epilogue
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      consumer_bar_sync();
-      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN + col0, 64, m_tile, r, []() {},
-                                                       stage_buf, store_groups, tr, k_begin == 0,
-                                                       FIXED_SPLIT ? sc.seg : 0);
+      // Epilogue, one column half at a time through this warpgroup's staging area. Barrier 3 + wg: no warp of the
+      // warpgroup still reads the area (previous half or tile) when it is rewritten, and all of it is written before
+      // any warp reads it.
+      bar_sync(3 + wg, 128);
+      gemm_stage_half<0>(acc_half, acc0, wl, lane);
+      gemm_stage_half<0>(acc_half + 64 * kAccCols, acc1, wl, lane);
+      bar_sync(3 + wg, 128);
+      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN, kAccCols, m_tile, r, []() {},
+                                                       stage_buf, store_groups, tr, kb == 0, seg);
+      bar_sync(3 + wg, 128);
+      gemm_stage_half<1>(acc_half, acc0, wl, lane);
+      gemm_stage_half<1>(acc_half + 64 * kAccCols, acc1, wl, lane);
+      bar_sync(3 + wg, 128);
+      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN + kAccCols, kAccCols, m_tile, r,
+                                                       []() {}, stage_buf, store_groups, tr, kb == 0, seg);
       tr(7);
     }
     if (EPI != EPI_DIRECT && elect_one_sync()) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem

@@ -11,7 +11,7 @@
  *     except where stated;
  *   - every function returns 0 on success, non-zero on failure; lseg_last_error() returns a
  *     thread-local message. There is NO CPU fallback: without a CUDA device of compute capability
- *     10.0 every compute entry point fails.
+ *     9.0 every compute entry point fails.
  *   - fp16 tensors are IEEE binary16 ("half"); int64 tokens match clip.tokenize's LongTensor [K,77].
  */
 #ifndef LSEG_B200_H_
@@ -40,6 +40,9 @@ enum { LSEG_ACT_NONE = 0, LSEG_ACT_GELU = 1, LSEG_ACT_QUICKGELU = 2, LSEG_ACT_RE
 enum { LSEG_STORE_ROWMAJOR = 0, LSEG_STORE_D2S = 1, LSEG_STORE_NCHW_T = 2 };
 
 /* One dense contraction  C[M,N] = epi(A[M,K] * W[N,K]^T)  on wgmma (k1,k4,k6-k8,k10-k17,k19).
+ * K must be a multiple of 64 and a row-major ldc a multiple of 8. bias, scale, res_f32, res2_f32, res_f16, out_f32, out_f16
+ * and out_f16_relu must be 16-byte aligned (the epilogue moves them with 16-byte vector accesses); lseg_gemm rejects a
+ * call that breaks one of these rules with an error naming the operand, before it touches any memory.
  * Replaces the torch Linear / Conv2d(1x1, 3x3 s1 p1) / ConvTranspose2d(k==s) calls listed in
  * SURVEY.md section 8(a): timm Block linears (lseg_vit.py:196-197), ProjectReadout (lseg_vit.py:79-90),
  * act_postprocess convs (lseg_vit.py:450-522), scratch.layerN_rn (lseg_blocks.py:73-108),
@@ -83,6 +86,15 @@ typedef struct lseg_gemm_args {
                          * identity), the ResNet-101 zero-shot trunk lseg_net_zs.py:307-310); row-major store, needs res_f32 */
 } lseg_gemm_args;
 int lseg_gemm(const lseg_gemm_args* args, void* stream);
+/* Debug: plans the GEMM lseg_gemm would run for `args` (same checks, same error messages) without launching anything or
+ * allocating, and describes the plan in out[5] (host):
+ *   out[0] epilogue: 0 register-direct, 1 TMA fp16 store, 2 TMA fp32 reduce-add;
+ *   out[1] grid (CTAs);
+ *   out[2] 1 if stream-K balancing splits tiles' K ranges over CTAs (reduce-add epilogue, lseg_set_deterministic(0));
+ *   out[3] fixed split-K segment count (>= 2: raw partials + a reduce kernel), 0 otherwise;
+ *   out[4] kernel instantiation: 0 register-direct, 1 TMA fp16, 2 TMA reduce-add, 3 fixed split-K, 4 grouped NCHW store
+ *          (nchw_group > 0), 5 ReLU after the fp32 residual. */
+int lseg_debug_gemm_plan(const lseg_gemm_args* args, int out[5]);
 
 /* Fused MHSA, head_dim 64 (k5; timm Attention restated at lseg_vit.py:26-39; CLIP text MHA).
  * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64]. */
@@ -97,8 +109,8 @@ int lseg_mhsa_variant(const void* qkv, void* out, int B, int N, int heads, int c
  * CTA per (label, head). qkv fp16 [K, L, 3*heads*64] -> out fp16 [K*L, heads*64], L <= 80. */
 int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* stream);
 /* 1 (default): every floating-point sum is formed in a fixed order (bit-reproducible across runs and batch sizes).
- * 0 (or LSEG_SPLITK=1): the in-place residual GEMM of the MLP (fc2) may split a tile's K range over two CTAs whose
- * partial sums are reduce-added in arrival order (differences at the fp32 rounding level, hence off by default). */
+ * 0 (or LSEG_SPLITK=1): an in-place fp32 residual GEMM without an activation (the MLP's fc2) may split a tile's K range
+ * over two CTAs whose partial sums are reduce-added in arrival order (differences at the fp32 rounding level, hence off by default). */
 int lseg_set_deterministic(int on);
 /* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTAs
  * into trace ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). Row w of a CTA is

@@ -345,8 +345,9 @@ __device__ __forceinline__ float exp2_poly(float x) {
 
 // Exact-erf GELU x * Phi(x) with Phi(x) = 1 / (1 + 2^(x * P(x^2))): P is a degree-4 minimax fit (tools/fit_gelu.py:
 // reweighted least squares against scipy erfc on [-7, 7], coefficients carry the -log2(e)); |gelu error| <= 3.7e-6 over
-// all x in fp32 arithmetic, i.e. below the fp16 rounding of the stored activation wherever that activation is
-// not already in fp16's subnormal range. 10 issue slots (2 MUFU) instead of the 20 of the Abramowitz-Stegun
+// all x in fp32 arithmetic (plus the rounding of the final product x * r at large |x|). That is below half an fp16 ulp
+// only where |gelu(x)| >= 2^-7: a smaller activation (the negative tail below x = -2.7) stored in fp16 can be off by
+// more than one fp16 ulp, by at most 3.7e-6 plus its rounding (measured, tests/test_gemm_exact_gpu.py). 10 issue slots (2 MUFU) instead of the 20 of the Abramowitz-Stegun
 // 7.1.26 form used before (the fc1 epilogue is issue-bound). P(u) < 0 for all u >= 0, so the sigmoid saturates
 // monotonically outside the fitted range.
 __device__ __forceinline__ float gelu_erf(float x) {

@@ -109,7 +109,8 @@ struct GemmTrace {
 
 // ------------------------------------------------------------------------------------------
 // Epilogue math of one 32-column chunk of one output row: f = act(v * scale + bias), plus the optional
-// partial squared row norm. v = the row's fp32 accumulators for columns [n0, n0+32).
+// partial squared row norm. v = the row's fp32 accumulators for columns [n0, n0+32). use_bias = false: a stream-K
+// segment that does not start at k = 0 (its partial sum is reduce-added to the one that carries the bias).
 // ------------------------------------------------------------------------------------------
 // Per-column constants of the (up to) 128 columns a warp handles in one tile, held in registers: lane l keeps
 // columns 4l..4l+3 (zeros beyond N), fetched with ONE coalesced 16-byte load per lane before the accumulator is
@@ -158,8 +159,8 @@ __device__ __forceinline__ void gemm_epilogue_math(const GemmEpi& e, int N, cons
         f[4 * j + 3] += __shfl_sync(0xffffffffu, cc.bias.w, src);
       }
     }
-  } else if (nvalid == 32) {  // uniform-address 16 B loads: one broadcast transaction each
-    if (e.scale) {
+  } else if (nvalid == 32 && (N & 3) == 0) {  // uniform-address 16 B loads: one broadcast transaction each (a grouped
+    if (e.scale) {                             // bias row starts at group * N: 16-byte aligned only when N % 4 == 0)
       const float4* sp = reinterpret_cast<const float4*>(e.scale + n0);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -167,7 +168,7 @@ __device__ __forceinline__ void gemm_epilogue_math(const GemmEpi& e, int N, cons
         f[4 * j] *= s.x; f[4 * j + 1] *= s.y; f[4 * j + 2] *= s.z; f[4 * j + 3] *= s.w;
       }
     }
-    if (e.bias) {
+    if (e.bias && use_bias) {
       const float4* bp = reinterpret_cast<const float4*>(e.bias + bias_off + n0);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -180,7 +181,7 @@ __device__ __forceinline__ void gemm_epilogue_math(const GemmEpi& e, int N, cons
 #pragma unroll
       for (int i = 0; i < 32; ++i) f[i] *= (i < nvalid) ? __ldg(e.scale + n0 + i) : 0.f;
     }
-    if (e.bias) {
+    if (e.bias && use_bias) {
       const float* bp = e.bias + bias_off + n0;
 #pragma unroll
       for (int i = 0; i < 32; ++i) f[i] += (i < nvalid) ? __ldg(bp + i) : 0.f;

@@ -222,6 +222,22 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     set_error("gemm: K=%d must be a multiple of %d", d.K, kGemmBK);
     return -1;
   }
+  {  // the epilogue reads and writes these operands with 16-byte vector accesses
+    const struct { const void* ptr; const char* name; } ops[] = {
+        {d.e.bias, "bias"}, {d.e.scale, "scale"}, {d.e.res_f32, "res_f32"}, {d.e.res2_f32, "res2_f32"},
+        {d.e.res_f16, "res_f16"}, {d.e.out_f32, "out_f32"}, {d.e.out_f16, "out_f16"},
+        {d.e.out_f16_relu, "out_f16_relu"}};
+    for (const auto& op : ops) {
+      if ((reinterpret_cast<uintptr_t>(op.ptr) & 15) != 0) {
+        set_error("gemm: %s pointer %p is not 16-byte aligned", op.name, op.ptr);
+        return -1;
+      }
+    }
+  }
+  if (d.e.relu_after_res && (d.e.store != STORE_ROWMAJOR || !d.e.res_f32 || d.e.res_f16 || d.e.out_row_sumsq)) {
+    set_error("gemm: relu_after_res needs a row-major store and an fp32 residual");
+    return -1;
+  }
   const int taps = d.conv ? d.kh * d.kw : 1;
   const long long ktot = static_cast<long long>(taps) * d.K;
   if (d.w_rows < kGemmBN && d.w_rows < d.N) {
@@ -292,10 +308,6 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     const GemmEpi& e = p.e;
     static const bool disabled = getenv("LSEG_GEMM_NO_TMA_STORE") != nullptr;
     const bool rowmajor = !disabled && e.store == STORE_ROWMAJOR && (d.N % 8 == 0) && d.N >= 64;
-    if (e.relu_after_res && (e.store != STORE_ROWMAJOR || !e.res_f32 || e.res_f16 || e.out_row_sumsq)) {
-      set_error("gemm: relu_after_res needs a row-major store and an fp32 residual");
-      return -1;
-    }
     if (rowmajor && e.out_f16 && !e.out_f32 && !e.out_f16_relu && !e.res_f16 && !e.res_f32 && !e.res2_f32 &&
         (e.ldc % 8 == 0)) {
       if (d.conv) {
@@ -318,10 +330,11 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
       const uint32_t box[2] = {32, 32};
       if (make_tmap(&p.tma_c, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, e.out_f32, 2, dims, str, box)) return -1;
       plan->epi = EPI_TMA_ADD;
-      // stream-K style balancing when whole tiles would leave a ragged last wave
+      // stream-K style balancing when whole tiles would leave a ragged last wave. Only without an activation: the
+      // segments of a tile reduce-add their epilogue results, and act(p1 + p2 + b) != act(p1 + b) + act(p2).
       static const int min_kit = getenv("LSEG_SPLITK_MIN_KITERS") ? atoi(getenv("LSEG_SPLITK_MIN_KITERS")) : 32;
-      p.split_k =
-          (!g_deterministic && tiles > g_num_sms && tiles % g_num_sms != 0 && p.k_iters >= min_kit) ? 1 : 0;
+      p.split_k = (!g_deterministic && e.act == ACT_NONE && tiles > g_num_sms && tiles % g_num_sms != 0 &&
+                   p.k_iters >= min_kit) ? 1 : 0;
     }
   }
   plan->grid = tiles < g_num_sms ? tiles : g_num_sms;
@@ -354,16 +367,27 @@ static int gemm_run(const GemmPlan& plan, cudaStream_t stream) {
   }
   return gemm_run_kernel(plan, stream);
 }
+// Which gemm_tc_kernel instantiation runs a plan (numbering of lseg_debug_gemm_plan's out[4]).
+enum GemmKernel { GK_DIRECT = 0, GK_TMA_F16 = 1, GK_TMA_ADD = 2, GK_FIXED_SPLIT = 3, GK_GROUPED_NCHW = 4, GK_RELU_RES = 5 };
+static int gemm_kernel_of(const GemmPlan& plan) {
+  if (plan.epi == EPI_TMA_F16) return GK_TMA_F16;
+  if (plan.epi == EPI_TMA_ADD) return GK_TMA_ADD;
+  if (plan.p.split_fixed > 1) return GK_FIXED_SPLIT;
+  if (plan.p.e.store == STORE_NCHW_T && plan.p.e.nchw_group > 0) return GK_GROUPED_NCHW;
+  if (plan.p.e.relu_after_res) return GK_RELU_RES;
+  return GK_DIRECT;
+}
 static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream) {
 #define LSEG_LAUNCH(KERNEL, EPI_) \
   launch_pdl(KERNEL, dim3(plan.grid), dim3(GemmCfg<EPI_>::kThreads), GemmCfg<EPI_>::kSmemBytes, stream, plan.p)
-  if (plan.epi == EPI_TMA_F16) LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_F16>, EPI_TMA_F16);
-  else if (plan.epi == EPI_TMA_ADD) LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_ADD>, EPI_TMA_ADD);
-  else if (plan.p.split_fixed > 1) LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT);
-  else if (plan.p.e.store == STORE_NCHW_T && plan.p.e.nchw_group > 0)
-    LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT);
-  else if (plan.p.e.relu_after_res) LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT);
-  else LSEG_LAUNCH(gemm_tc_kernel<EPI_DIRECT>, EPI_DIRECT);
+  switch (gemm_kernel_of(plan)) {
+    case GK_TMA_F16: LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_F16>, EPI_TMA_F16); break;
+    case GK_TMA_ADD: LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_ADD>, EPI_TMA_ADD); break;
+    case GK_FIXED_SPLIT: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT); break;
+    case GK_GROUPED_NCHW: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT); break;
+    case GK_RELU_RES: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT); break;
+    default: LSEG_LAUNCH(gemm_tc_kernel<EPI_DIRECT>, EPI_DIRECT); break;
+  }
 #undef LSEG_LAUNCH
   LSEG_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -487,12 +511,11 @@ static void fill_epi(const lseg_gemm_args* a, GemmEpi* e) {
   e->relu_after_res = a->relu_after_res;
 }
 
-int lseg_gemm(const lseg_gemm_args* a, void* stream) {
+static int gemm_desc_of(const lseg_gemm_args* a, GemmDesc& d) {
   if (!a) {
     set_error("lseg_gemm: null args");
     return -1;
   }
-  GemmDesc d;
   memset(&d, 0, sizeof(d));
   d.a = static_cast<const __half*>(a->a);
   d.lda = a->lda;
@@ -509,6 +532,12 @@ int lseg_gemm(const lseg_gemm_args* a, void* stream) {
   d.kh = d.kw = a->ksize;
   d.pad = a->pad;
   fill_epi(a, &d.e);
+  return 0;
+}
+
+int lseg_gemm(const lseg_gemm_args* a, void* stream) {
+  GemmDesc d;
+  if (gemm_desc_of(a, d)) return -1;
   GemmPlan plan;
   if (gemm_plan(d, &plan)) return -1;
   if (plan.ws_bytes) {  // stage-op call: a per-device scratch that only grows (the engine plans own theirs)
@@ -705,6 +734,19 @@ int lseg_set_deterministic(int on) {
   if (ensure_init()) return -1;
   if ((on != 0) != (g_deterministic != 0)) ++g_plan_epoch;
   g_deterministic = on ? 1 : 0;
+  return 0;
+}
+
+int lseg_debug_gemm_plan(const lseg_gemm_args* a, int out[5]) {
+  GemmDesc d;
+  if (gemm_desc_of(a, d)) return -1;
+  GemmPlan plan;
+  if (gemm_plan(d, &plan)) return -1;
+  out[0] = plan.epi;
+  out[1] = plan.grid;
+  out[2] = plan.p.split_k;
+  out[3] = plan.p.split_fixed;
+  out[4] = gemm_kernel_of(plan);
   return 0;
 }
 

@@ -46,11 +46,10 @@ def read_watchdog():
     return list(arr)
 
 
-def gemm(a, w, N=None, *, bias=None, bias_group_rows=0, scale=None, act=ACT_NONE, res_f32=None, res2_f32=None,
-         res_f16=None, out_f32=None, out_f16=None, out_f16_relu=None, ldc=None, M=None,
-         conv=None, store=STORE_ROWMAJOR, d2s=None, nchw=None, row_sumsq=None, row_scale=1.0, out_row_sumsq=None,
-         relu_after_res=False):
-    """C = epi(A W^T).  a: fp16 [M,K] (or NHWC [B,H,W,C] when conv=(ksize,pad)); w: fp16 [rows>=N, Ktot]."""
+def _gemm_args(a, w, N=None, *, bias=None, bias_group_rows=0, scale=None, act=ACT_NONE, res_f32=None, res2_f32=None,
+               res_f16=None, out_f32=None, out_f16=None, out_f16_relu=None, ldc=None, M=None,
+               conv=None, store=STORE_ROWMAJOR, d2s=None, nchw=None, row_sumsq=None, row_scale=1.0, out_row_sumsq=None,
+               relu_after_res=False):
     args = GemmArgs()
     args.a = _ptr(a, torch.float16)
     args.w = _ptr(w, torch.float16)
@@ -87,7 +86,21 @@ def gemm(a, w, N=None, *, bias=None, bias_group_rows=0, scale=None, act=ACT_NONE
     args.row_scale = float(row_scale)
     args.out_row_sumsq = _ptr(out_row_sumsq, torch.float32)
     args.relu_after_res = int(bool(relu_after_res))
-    check(load().lseg_gemm(C.byref(args), _stream()))
+    return args
+
+
+def gemm(a, w, N=None, **kw):
+    """C = epi(A W^T).  a: fp16 [M,K] (or NHWC [B,H,W,C] when conv=(ksize,pad)); w: fp16 [rows>=N, Ktot].
+    Keywords: see _gemm_args and lseg_gemm_args in include/lseg_b200.h."""
+    check(load().lseg_gemm(C.byref(_gemm_args(a, w, N, **kw)), _stream()))
+
+
+def gemm_plan(a, w, N=None, **kw):
+    """The plan gemm(a, w, N, **kw) would run, without running it (include/lseg_b200.h lseg_debug_gemm_plan):
+    dict with epi (0 direct, 1 TMA fp16, 2 TMA reduce-add), grid, split_k, split_fixed and kernel (instantiation)."""
+    out = (C.c_int * 5)()
+    check(load().lseg_debug_gemm_plan(C.byref(_gemm_args(a, w, N, **kw)), C.byref(out)))
+    return dict(zip(("epi", "grid", "split_k", "split_fixed", "kernel"), out))
 
 
 def mhsa(qkv, B, N, heads, causal=False, variant=None, out=None):

@@ -59,9 +59,9 @@ def test_gemm_bias_f32_f16(ops, M, N, K):
 
 @pytest.mark.parametrize("M,N,K", [(7208, 1024, 1024), (7208, 1024, 4096), (8468, 1024, 1024), (300, 1024, 512)])
 def test_gemm_inplace_residual_tile_widths(ops, M, N, K):
-    """x += A W^T + b through the bulk reduce-add epilogue at the ViT shapes: B=8 480^2 (29 row pairs -> the planner picks
-    224-wide tiles: 145 pair tiles = 1.96 waves), B=4 736^2 (34 row pairs -> 256-wide), and a single-wave case. The column
-    split of the 224-wide tile (128 | 96 per epilogue warp pair, last tile 128 valid columns) must cover every column."""
+    """x += A W^T + b through the bulk reduce-add epilogue at the ViT shapes: B=8 480^2 (57 x 8 = 456 tiles of 128 x 128:
+    3.45 waves on 132 SMs, an M tail of 40 rows), the same with K = 4096, B=4 736^2 (67 x 8 = 536 tiles, a 20-row tail),
+    and a single-wave case (3 x 8 tiles)."""
     a = _rand((M, K), 41, 0.5)
     w = _rand((N, K), 42, 0.03)
     bias = _rand((N,), 43, 0.5, torch.float32)
@@ -274,7 +274,7 @@ def _mhsa_ref(qkv, B, N, heads, causal):
 
 MHSA_SHAPES = [
     (2, 901, 16, False, 1.0), (3, 77, 8, True, 1.0), (1, 37, 16, False, 1.0), (1, 300, 2, True, 1.0),
-    # tile-boundary cases of the 64-key two-stream kernels: one tile only (second stream empty), exact multiples,
+    # key-tile boundary cases of the wgmma flash-attention kernel (64 keys per K/V tile): a single tile, exact multiples,
     # 1..2 keys in the tail tile, odd/even tile counts; amp 3 makes the running-max offset move (O rescale path)
     (1, 64, 1, False, 1.0), (1, 65, 1, True, 1.0), (1, 128, 2, False, 1.0), (1, 130, 2, False, 3.0),
     (1, 1025, 2, False, 1.0), (2, 300, 2, False, 3.0), (1, 193, 1, True, 3.0),

@@ -97,7 +97,10 @@ int lseg_gemm(const lseg_gemm_args* args, void* stream);
 int lseg_debug_gemm_plan(const lseg_gemm_args* args, int out[5]);
 
 /* Fused MHSA, head_dim 64 (k5; timm Attention restated at lseg_vit.py:26-39; CLIP text MHA).
- * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64]. */
+ * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64].
+ * B, N and heads must be positive with B*heads <= 65535; qkv must be 16-byte aligned (TMA loads) and out 4-byte aligned
+ * (__half2 stores). lseg_mhsa, lseg_mhsa_variant and lseg_mhsa_trace reject a call that breaks one of these rules with an
+ * error naming the argument, before anything is launched. */
 int lseg_mhsa(const void* qkv, void* out, int B, int N, int heads, int causal, void* stream);
 /* Same contract as lseg_mhsa with an explicit kernel choice (A/B measurements; the engine runs variant 0 unless
  * LSEG_MHSA_VARIANT overrides it). One wgmma flash-attention kernel; the variants differ in how many exponentials are
@@ -106,7 +109,9 @@ int lseg_mhsa(const void* qkv, void* out, int B, int N, int heads, int causal, v
 int lseg_mhsa_variant(const void* qkv, void* out, int B, int N, int heads, int causal, int variant, void* stream);
 /* Causal attention of the CLIP text tower with the rounding points of torch's multi_head_attention_forward on fp16
  * tensors (q*dh^-0.5, bmm -> fp16, softmax -> fp16 normalised, bmm -> fp16; SURVEY.md Appendix A.2): CUDA cores, one
- * CTA per (label, head). qkv fp16 [K, L, 3*heads*64] -> out fp16 [K*L, heads*64], L <= 80. */
+ * CTA per (label, head). qkv fp16 [K, L, 3*heads*64] -> out fp16 [K*L, heads*64]. 1 <= L <= 80, 1 <= K <= 65535 and
+ * 1 <= heads <= 65535; qkv and out must be 4-byte aligned (__half2 loads and stores). A call that breaks one of these
+ * rules is rejected with an error naming the argument, before anything is launched. */
 int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* stream);
 /* 1 (default): every floating-point sum is formed in a fixed order (bit-reproducible across runs and batch sizes).
  * 0 (or LSEG_SPLITK=1): an in-place fp32 residual GEMM without an activation (the MLP's fc2) may split a tile's K range
@@ -117,8 +122,9 @@ int lseg_set_deterministic(int on);
  * warp w: rows 4-7 are consumer warpgroup 0 and rows 8-11 warpgroup 1, each stamping only the tiles it owns (every
  * other entry of the CTA's work list); the other rows stay zero. Stamp = clock64() << 8 | tag. */
 int lseg_debug_gemm_trace(unsigned long long* trace);
-/* Debug: same computation, additionally stamps clock64() at the pipeline hand-off points of 16 sampled CTAs into
- * trace ([16][10 warps][256] uint64 device memory, zero-initialised by the caller). */
+/* Debug: same computation and rules as lseg_mhsa (variant 0), additionally stamps clock64() at the pipeline hand-off
+ * points of 16 sampled CTAs into trace ([16][10 warps][256] uint64 device memory, zero-initialised by the caller,
+ * not NULL). */
 int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int causal, unsigned long long* trace,
                     void* stream);
 

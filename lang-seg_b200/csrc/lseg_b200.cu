@@ -402,6 +402,30 @@ struct MhsaPlan {
 };
 static int mhsa_plan(const MhsaDesc& d, MhsaPlan* plan) {
   if (ensure_init()) return -1;
+  // the rules of include/lseg_b200.h, checked before a tensor map is encoded: one CTA row per (image, head) in
+  // gridDim.y, TMA loads of qkv (16-byte base) and __half2 stores to out (4-byte base)
+  {
+    const struct { int v; const char* name; } dims[] = {{d.B, "B"}, {d.N, "N"}, {d.heads, "heads"}};
+    for (const auto& x : dims) {
+      if (x.v <= 0) {
+        set_error("mhsa: %s=%d must be positive", x.name, x.v);
+        return -1;
+      }
+    }
+  }
+  if (static_cast<long long>(d.B) * d.heads > 65535) {
+    set_error("mhsa: B*heads = %lld exceeds 65535 (B=%d, heads=%d)", static_cast<long long>(d.B) * d.heads, d.B,
+              d.heads);
+    return -1;
+  }
+  if (!d.qkv || (reinterpret_cast<uintptr_t>(d.qkv) & 15) != 0) {
+    set_error("mhsa: qkv pointer %p is null or not 16-byte aligned", static_cast<const void*>(d.qkv));
+    return -1;
+  }
+  if (!d.out || (reinterpret_cast<uintptr_t>(d.out) & 3) != 0) {
+    set_error("mhsa: out pointer %p is null or not 4-byte aligned", static_cast<const void*>(d.out));
+    return -1;
+  }
   MhsaParams& p = plan->p;
   memset(&p, 0, sizeof(p));
   const int D = d.heads * kMhsaDh;
@@ -757,6 +781,10 @@ int lseg_debug_gemm_trace(unsigned long long* trace) {
 
 int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int causal, unsigned long long* trace,
                     void* stream) {
+  if (!trace) {
+    set_error("mhsa_trace: trace pointer is null");
+    return -1;
+  }
   MhsaDesc d;
   d.qkv = static_cast<const __half*>(qkv);
   d.out = static_cast<__half*>(out);

@@ -96,8 +96,25 @@ __global__ void __launch_bounds__(kTaWarps * 32) text_attn_kernel(const __half* 
 }
 
 static inline int launch_text_attn(const __half* qkv, __half* out, int K, int L, int heads, cudaStream_t s) {
-  if (L > kTaMaxL || L <= 0 || K <= 0 || K > 65535) {
-    set_error("text_attn: bad shape K=%d L=%d", K, L);
+  if (L > kTaMaxL || L <= 0) {
+    set_error("text_attn: L=%d must be in 1..%d", L, kTaMaxL);
+    return -1;
+  }
+  if (K <= 0 || K > 65535) {
+    set_error("text_attn: K=%d must be in 1..65535", K);
+    return -1;
+  }
+  if (heads <= 0 || heads > 65535) {
+    set_error("text_attn: heads=%d must be in 1..65535", heads);
+    return -1;
+  }
+  // __half2 loads and stores
+  if (!qkv || (reinterpret_cast<uintptr_t>(qkv) & 3) != 0) {
+    set_error("text_attn: qkv pointer %p is null or not 4-byte aligned", static_cast<const void*>(qkv));
+    return -1;
+  }
+  if (!out || (reinterpret_cast<uintptr_t>(out) & 3) != 0) {
+    set_error("text_attn: out pointer %p is null or not 4-byte aligned", static_cast<const void*>(out));
     return -1;
   }
   launch_pdl(text_attn_kernel, dim3(heads, K), dim3(kTaWarps * 32), 0, s, qkv, out, L, heads);

@@ -103,10 +103,19 @@ def gemm_plan(a, w, N=None, **kw):
     return dict(zip(("epi", "grid", "split_k", "split_fixed", "kernel"), out))
 
 
-def mhsa(qkv, B, N, heads, causal=False, variant=None, out=None):
-    """variant=None: the kernel the engine runs; 0..4: see lseg_mhsa_variant in include/lseg_b200.h."""
+def _attn_out(out, rows, heads, device, what):
+    """A caller-given output must be fp16 [rows, heads*64]: the kernel writes exactly that much, unchecked."""
     if out is None:
-        out = torch.empty((B * N, heads * 64), dtype=torch.float16, device=qkv.device)
+        return torch.empty((rows, heads * 64), dtype=torch.float16, device=device)
+    if out.dtype != torch.float16 or tuple(out.shape) != (rows, heads * 64):
+        raise _lib.LsegError(f"{what}: out must be fp16 [{rows}, {heads * 64}], got {out.dtype} {list(out.shape)}")
+    return out
+
+
+def mhsa(qkv, B, N, heads, causal=False, variant=None, out=None):
+    """variant=None: the kernel the engine runs; 0..8: see lseg_mhsa_variant in include/lseg_b200.h.
+    out: optional fp16 [B*N, heads*64]."""
+    out = _attn_out(out, B * N, heads, qkv.device, "mhsa")
     if variant is None:
         check(load().lseg_mhsa(_ptr(qkv, torch.float16), _ptr(out), B, N, heads, int(causal), _stream()))
     else:
@@ -115,9 +124,10 @@ def mhsa(qkv, B, N, heads, causal=False, variant=None, out=None):
     return out
 
 
-def text_attn(qkv, K, L, heads):
-    """Causal CLIP-text attention with torch's fp16 rounding points (include/lseg_b200.h lseg_text_attn)."""
-    out = torch.empty((K * L, heads * 64), dtype=torch.float16, device=qkv.device)
+def text_attn(qkv, K, L, heads, out=None):
+    """Causal CLIP-text attention with torch's fp16 rounding points (include/lseg_b200.h lseg_text_attn).
+    out: optional fp16 [K*L, heads*64]."""
+    out = _attn_out(out, K * L, heads, qkv.device, "text_attn")
     check(load().lseg_text_attn(_ptr(qkv, torch.float16), _ptr(out), K, L, heads, _stream()))
     return out
 
@@ -164,9 +174,9 @@ def set_deterministic(on):
     check(load().lseg_set_deterministic(int(bool(on))))
 
 
-def mhsa_trace(qkv, B, N, heads, causal=False):
-    """Debug: (out, trace[16 CTAs, 10 warps, 256]) with clock64 << 8 | tag stamps."""
-    out = torch.empty((B * N, heads * 64), dtype=torch.float16, device=qkv.device)
+def mhsa_trace(qkv, B, N, heads, causal=False, out=None):
+    """Debug: (out, trace[16 CTAs, 10 warps, 256]) with clock64 << 8 | tag stamps. out: optional fp16 [B*N, heads*64]."""
+    out = _attn_out(out, B * N, heads, qkv.device, "mhsa_trace")
     trace = torch.zeros((16, 10, 256), dtype=torch.int64, device=qkv.device)
     check(load().lseg_mhsa_trace(_ptr(qkv, torch.float16), _ptr(out), B, N, heads, int(causal), _ptr(trace), _stream()))
     return out, trace

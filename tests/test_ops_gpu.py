@@ -5,10 +5,13 @@ accumulation is fp32 on both sides -> differences come only from summation order
 to the output scale) plus one fp16 rounding where the output is fp16 (2^-11 relative).
 """
 import math
+import os
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+from attention_oracle import EPS_EX2, EPS_POLY, MHSA_SHAPES, mhsa_oracle, violations
 
 pytestmark = pytest.mark.gpu
 
@@ -31,6 +34,10 @@ def _watchdog(ops):
 def _rand(shape, seed, scale=1.0, dtype=torch.float16):
     g = torch.Generator(device="cpu").manual_seed(seed)
     return (torch.randn(shape, generator=g) * scale).to(dtype).cuda()
+
+
+def _env_variant():
+    return int(os.environ.get("LSEG_MHSA_VARIANT", "0"))
 
 
 def _close(got, ref, tol, what):
@@ -272,16 +279,6 @@ def _mhsa_ref(qkv, B, N, heads, causal):
     return (s.softmax(-1) @ v).transpose(1, 2).reshape(B * N, D)
 
 
-MHSA_SHAPES = [
-    (2, 901, 16, False, 1.0), (3, 77, 8, True, 1.0), (1, 37, 16, False, 1.0), (1, 300, 2, True, 1.0),
-    # key-tile boundary cases of the wgmma flash-attention kernel (64 keys per K/V tile): a single tile, exact multiples,
-    # 1..2 keys in the tail tile, odd/even tile counts; amp 3 makes the running-max offset move (O rescale path)
-    (1, 64, 1, False, 1.0), (1, 65, 1, True, 1.0), (1, 128, 2, False, 1.0), (1, 130, 2, False, 3.0),
-    (1, 1025, 2, False, 1.0), (2, 300, 2, False, 3.0), (1, 193, 1, True, 3.0),
-    # token counts of BASELINE.json configs[4]: 704^2 -> 1937, 736^2 -> 2117 (34 key tiles; 17 query tiles)
-    (1, 1937, 4, False, 1.0), (1, 2117, 3, False, 1.0), (1, 2117, 1, False, 3.0)]
-
-
 # variant None = the kernel the engine runs; 0..8 = every number lseg_mhsa_variant accepts: 0/1/2/5/6 all exponentials
 # on the MUFU pipe, 3/7 one of four score pairs on the FMA pipe, 4/8 two of four (include/lseg_b200.h)
 @pytest.mark.parametrize("variant", [None, 0, 1, 2, 3, 4, 5, 6, 7, 8])
@@ -291,6 +288,12 @@ def test_mhsa(ops, B, N, heads, causal, amp, variant):
     qkv = _rand((B, N, 3 * D), 19, amp)
     out = ops.mhsa(qkv, B, N, heads, causal, variant=variant)
     _close(out, _mhsa_ref(qkv, B, N, heads, causal), 2e-3, f"mhsa variant {variant}")
+    # and element by element within the float64 bound of tests/attention_oracle.py (tests/test_attention_gpu.py has
+    # the full sweep)
+    poly = (_env_variant() if variant is None else variant) in (3, 4, 7, 8)
+    ref, bound = mhsa_oracle(qkv, B, N, heads, causal, EPS_POLY if poly else EPS_EX2)
+    n, msg = violations(out, ref, bound)
+    assert n == 0, f"mhsa variant {variant}: {msg}"
 
 
 def test_text_attn_rounding_points(ops):

@@ -29,7 +29,9 @@ extern "C" {
 const char* lseg_last_error(void);
 int lseg_abi_version(void);
 /* Reads and clears the device-side barrier watchdog: out[0] != 0 means a kernel timed out on an
- * mbarrier (out[0] = wait tag, out[1] = block, out[2] = thread, out[3] = parity). Synchronises stream. */
+ * mbarrier (out[0] = wait tag, out[1] = block, out[2] = thread, out[3] = parity). Synchronises stream.
+ * When no barrier timed out it reports instead the first image whose metric group id was outside [0, G) since the last
+ * read (section "segmentation metrics"): out[0] = 78, out[1] = image, out[2] = its group id, out[3] = G. */
 int lseg_read_watchdog(int out[4], void* stream);
 
 /* ---- stage ops (each one is parity-tested on its own; SURVEY.md section 2b numbering) ------------ */
@@ -214,6 +216,30 @@ int lseg_eval_resize_add(const float* canvas, float* scores, int K, int height, 
 int lseg_preprocess(const unsigned char* img_hwc, float* out, int h, int w, int Ho, int Wo, int Hp, int Wp,
                     const float* mean3_host, const float* std3_host, const float* pad3_host, void* stream);
 
+/* ---- segmentation metrics: the counters behind pixAcc / mIoU (PyTorch-Encoding's SegmentationMetric, test_lseg.py:314-395)
+ * and the few-shot mIoU / FB-IoU (Evaluator.classify_prediction + AverageMeter, test_lseg_zs.py:290-316) -----------------
+ * stats is a caller buffer of G rows of int64 counters, 3*nclass + 2 per row:
+ *     [ inter(nclass) | pred(nclass) | label(nclass) | correct | labeled ]
+ * For every pixel of image b, with predicted class p and int64 target t, row g = group[b] (group: int32 [B], or NULL to
+ * count every image into row 0; rows may repeat and G may exceed B):
+ *     t < 0            : ignored (no counter changes)
+ *     otherwise        : labeled += 1
+ *       p == t         : correct += 1, and inter[t] += 1 if t < nclass
+ *       0 <= p < nclass: pred[p] += 1
+ *       t < nclass     : label[t] += 1
+ * union = pred + label - inter. The calls ADD to stats and never clear it. A target >= nclass (e.g. 255) counts as labeled
+ * and adds to pred only; a prediction >= nclass (K > nclass) adds to no histogram. An image whose group id lies outside
+ * [0, G) is skipped and reported by lseg_read_watchdog (tag 78). Rejected by name before any launch: NULL pointers, stats
+ * or target not 8-byte aligned, group not 4-byte aligned, nclass outside [1, 2^24], G <= 0, B outside [1, 65535],
+ * H or W <= 0. nclass <= 1364 counts in shared memory, larger nclass with global atomics (same result). */
+/* scores fp32 [B,K,H,W]: p = first maximal class (torch.max(scores, 1)[1] on NaN-free input; a NaN score never wins, a
+ * pixel whose scores are all NaN or -inf gets class 0). target int64 [B,H,W]. */
+int lseg_seg_stats_scores(const float* scores, const long long* target, const int* group, int B, int K, int H, int W,
+                          int nclass, int G, long long* stats, void* stream);
+/* pred int64 [B,H,W] (8-byte aligned): p = pred. */
+int lseg_seg_stats_mask(const long long* pred, const long long* target, const int* group, int B, int H, int W, int nclass,
+                        int G, long long* stats, void* stream);
+
 /* ---- peer memory: the logits gather (SURVEY.md section 8(e)), one process per GPU over NVLink 5 / NVSwitch ----------
  * Replaces the thread-per-GPU DataParallel gather of additional_utils/models.py:35-53. A rank allocates a buffer its peers
  * can map (CUDA IPC; the 64-byte handle travels through any host channel, e.g. torch.distributed.all_gather_object);
@@ -356,6 +382,14 @@ int lseg_forward_lowres(lseg_engine* e, const float* x, int B, int H, int W, con
  * The fp32 [B,K,H,W] logits are not materialised unless `logits` is non-NULL (then both are produced). */
 int lseg_forward_argmax(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
                         long long text_image_stride, long long* mask, float* logits, void* stream);
+
+/* lseg_forward_argmax with the metric counters of section "segmentation metrics" fused into the same output kernel:
+ * target int64 [B,H,W], group int32 [B] or NULL, stats int64 [G, 3*nclass + 2] (accumulated). The argmax p is the mask
+ * lseg_forward_argmax computes; `mask` (int64 [B,H,W]) and `logits` (fp32 [B,K,H,W]) are optional outputs, NULL to skip
+ * them. Needs W <= 1024 besides lseg_forward's rules; every argument is checked before the first launch. */
+int lseg_forward_segstats(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
+                          long long text_image_stride, const long long* target, const int* group, int nclass, int G,
+                          long long* stats, long long* mask, float* logits, void* stream);
 
 /* Same as lseg_forward, but brackets every kernel launch with CUDA events on `stream`, synchronises,
  * and returns per-launch device time (ms), kernel class (0 elementwise, 1 wgmma GEMM, 2 MHSA,

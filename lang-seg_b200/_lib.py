@@ -96,6 +96,7 @@ SYMBOLS = [
     "lseg_p2p_alloc", "lseg_p2p_open", "lseg_p2p_close", "lseg_p2p_free", "lseg_p2p_copy", "lseg_p2p_signal",
     "lseg_p2p_wait",
     "lseg_eval_make_crops", "lseg_eval_canvas", "lseg_eval_resize_add", "lseg_preprocess",
+    "lseg_seg_stats_scores", "lseg_seg_stats_mask", "lseg_forward_segstats",
 ]
 
 _lib = None
@@ -186,6 +187,13 @@ def load(build_if_missing=True):
     lib.lseg_eval_resize_add.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_preprocess.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]
+    lib.lseg_seg_stats_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.c_int, C.c_void_p, C.c_void_p]
+    lib.lseg_seg_stats_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        C.c_void_p, C.c_void_p]
+    lib.lseg_forward_segstats.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                          C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p]
     lib.lseg_last_launch_count.argtypes = [C.c_void_p]
     lib.lseg_forward_profiled.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                           C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_float),

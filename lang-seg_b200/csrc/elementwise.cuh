@@ -13,6 +13,11 @@ namespace lseg {
     LSEG_CHECK_CUDA(cudaGetLastError());      \
     return 0;                                 \
   } while (0)
+}  // namespace lseg
+
+#include "segstats.cuh"
+
+namespace lseg {
 
 // ------------------------------------------------------------------------------------------
 // patchify: x fp32 NCHW [B,3,H,W] -> A fp16 [B*gh*gw, 3*P*P], column = c*P*P + py*P + px, which is
@@ -796,19 +801,17 @@ static inline int launch_upsample2x_nchw_bg(const __half* x, float* y, long long
 // One warp = one output row of one image, all K classes in turn: the two source rows of class k are interpolated
 // vertically into a (double-buffered) smem line, then every lane updates the running (max, argmax) of its
 // lane + 32 j outputs, j < kArgJ. Output columns beyond 32*kArgJ are handled in further passes.
+// kStats adds the metric counters of segstats.cuh: per pass, each lane reads the targets of its kArgJ pixels (coalesced)
+// and counts them into the block's histogram (all 8 warps of a block belong to one image, hence one counter row), which
+// is flushed once per block; the mask store becomes optional (mask may be nullptr).
 // ------------------------------------------------------------------------------------------
 constexpr int kArgJ = 16;  // outputs per lane per pass (Wo <= 512 in one pass)
-template <typename TIn>
-__global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __restrict__ lr, long long* __restrict__ mask,
-                                                                int K, int H, int W) {
-  griddep_launch_dependents();
-  griddep_wait();
-  __shared__ __align__(16) float line[8][2][kUpMaxW];
+template <typename TIn, bool kStats>
+__device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr, long long* __restrict__ mask, int K, int H,
+                                                      int W, int b, int oy, int lane, float (*line)[kUpMaxW],
+                                                      const SegStatsArgs& st, int* hist, unsigned long long* grow,
+                                                      int& labeled, int& correct) {
   const int Ho = 2 * H, Wo = 2 * W;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.y;
-  const int oy = blockIdx.x * 8 + warp;
-  if (oy >= Ho) return;  // warp-uniform
   const float sh = (Ho > 1) ? static_cast<float>(H - 1) / (Ho - 1) : 0.f;
   const float sw = (Wo > 1) ? static_cast<float>(W - 1) / (Wo - 1) : 0.f;
   const float fy = sh * oy;
@@ -817,7 +820,7 @@ __global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __res
   const float ly = fy - y0, hy = 1.f - ly;
   const long long plane_sz = static_cast<long long>(H) * W;
   const TIn* img = lr + static_cast<long long>(b) * K * plane_sz;
-  long long* orow = mask + (static_cast<long long>(b) * Ho + oy) * Wo;
+  const long long row_off = (static_cast<long long>(b) * Ho + oy) * Wo;
   for (int ox0 = 0; ox0 < Wo; ox0 += 32 * kArgJ) {
     int xa[kArgJ], xb[kArgJ];
     float lx[kArgJ], best[kArgJ];
@@ -836,7 +839,7 @@ __global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __res
     for (int k = 0; k < K; ++k) {
       const TIn* r0 = img + k * plane_sz + static_cast<long long>(y0) * W;
       const TIn* r1 = img + k * plane_sz + static_cast<long long>(y1) * W;
-      float* v = line[warp][k & 1];
+      float* v = line[k & 1];
       for (int c = lane; c < W / 8; c += 32) {
         float fa[8], fb[8], o[8];
         load8_f32(r0 + 8 * c, fa);
@@ -857,6 +860,21 @@ __global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __res
       }
     }
     __syncwarp();
+    if constexpr (kStats) {
+      if (grow) {  // nullptr: the image's group id is out of range
+        const long long* trow = st.target + row_off;
+        long long t[kArgJ];
+#pragma unroll
+        for (int j = 0; j < kArgJ; ++j) {
+          const int ox = ox0 + lane + 32 * j;
+          t[j] = ox < Wo ? __ldg(trow + ox) : -1;
+        }
+#pragma unroll
+        for (int j = 0; j < kArgJ; ++j) seg_count_pixel(arg[j], t[j], st.nclass, hist, grow, labeled, correct);
+      }
+      if (!mask) continue;
+    }
+    long long* orow = mask + row_off;
 #pragma unroll
     for (int j = 0; j < kArgJ; ++j) {
       const int ox = ox0 + lane + 32 * j;
@@ -864,13 +882,55 @@ __global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __res
     }
   }
 }
-template <typename TIn>
-static inline int launch_upsample2x_argmax(const TIn* lr, long long* mask, int B, int K, int H, int W, cudaStream_t s) {
+template <typename TIn, bool kStats>
+__global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __restrict__ lr, long long* __restrict__ mask,
+                                                                int K, int H, int W, SegStatsArgs st) {
+  griddep_launch_dependents();
+  griddep_wait();
+  __shared__ __align__(16) float line[8][2][kUpMaxW];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.y;
+  const int oy = blockIdx.x * 8 + warp;
+  if constexpr (kStats) {
+    extern __shared__ int seg_hist[];
+    const int g = seg_group_row(st, b, blockIdx.x == 0 && threadIdx.x == 0);
+    if (g < 0 && !mask) return;  // block-uniform
+    unsigned long long* grow =
+        g < 0 ? nullptr : reinterpret_cast<unsigned long long*>(st.stats + static_cast<long long>(g) * (3 * st.nclass + 2));
+    int* hist = grow && st.nclass <= kSegSmemMaxClass ? seg_hist : nullptr;
+    seg_block_begin(hist, st.nclass);
+    int labeled = 0, correct = 0;
+    if (oy < 2 * H)  // warps past the last row still take part in the block's flush
+      upsample2x_argmax_row<TIn, true>(lr, mask, K, H, W, b, oy, lane, line[warp], st, hist, grow, labeled, correct);
+    if (grow) seg_block_finish(hist, grow, st.nclass, labeled, correct);
+  } else {
+    if (oy >= 2 * H) return;  // warp-uniform
+    int unused = 0;
+    upsample2x_argmax_row<TIn, false>(lr, mask, K, H, W, b, oy, lane, line[warp], st, nullptr, nullptr, unused, unused);
+  }
+}
+static inline int check_upsample2x_argmax(int B, int K, int H, int W) {
   if (W % 8 != 0 || W > kUpMaxW || B > 65535 || K <= 0) {
     set_error("upsample2x_argmax: needs W %% 8 == 0, W <= %d, B <= 65535, K > 0 (W=%d B=%d K=%d)", kUpMaxW, W, B, K);
     return -1;
   }
-  launch_pdl(upsample2x_argmax_kernel<TIn>, dim3((2 * H + 7) / 8, B), dim3(256), 0, s, lr, mask, K, H, W);
+  return 0;
+}
+template <typename TIn>
+static inline int launch_upsample2x_argmax(const TIn* lr, long long* mask, int B, int K, int H, int W, cudaStream_t s) {
+  if (check_upsample2x_argmax(B, K, H, W)) return -1;
+  launch_pdl(upsample2x_argmax_kernel<TIn, false>, dim3((2 * H + 7) / 8, B), dim3(256), 0, s, lr, mask, K, H, W,
+             SegStatsArgs{});
+  LSEG_LAUNCH_CHECK();
+}
+// The same output stage with the metric counters of `st` (mask optional): dynamic shared memory holds the block
+// histogram when st.nclass <= kSegSmemMaxClass.
+template <typename TIn>
+static inline int launch_upsample2x_segstats(const TIn* lr, long long* mask, int B, int K, int H, int W,
+                                             const SegStatsArgs& st, cudaStream_t s) {
+  if (check_upsample2x_argmax(B, K, H, W)) return -1;
+  launch_pdl(upsample2x_argmax_kernel<TIn, true>, dim3((2 * H + 7) / 8, B), dim3(256), seg_smem_bytes(st.nclass), s, lr,
+             mask, K, H, W, st);
   LSEG_LAUNCH_CHECK();
 }
 

@@ -26,6 +26,7 @@ struct CallCtx {
   __half* out_lr;        // optional target of the fp16 low-res logits [B,K,H/2,W/2] (the exact result of the reference's
                          // fp16 matmul, lseg_net.py:194-196) instead of the plan's own buffer; may be PEER memory — the
                          // pixel x text GEMM then stores straight into another GPU's gather buffer over NVLink
+  const SegStatsArgs* seg = nullptr;  // optional metric counters, fused with the argmax output stage (out_mask optional)
 };
 using StepFn = std::function<int(const CallCtx&, cudaStream_t)>;
 enum StepKind { KIND_EW = 0, KIND_GEMM = 1, KIND_MHSA = 2, KIND_LN = 3, KIND_MEMSET = 4 };
@@ -909,7 +910,17 @@ static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W
     }
   }
   // ---- fused output_conv + torch.max(.., 1)[1] (SURVEY.md 8(f) row 2): the fp32 logits are never materialised ----
-  if (ctx.out_mask) {
+  if (ctx.seg) {  // ... and counted into the metric rows in the same kernel
+    if (lr32 ? launch_upsample2x_segstats(lr32, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream)
+             : launch_upsample2x_segstats(lr, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream))
+      return -1;
+    ++launches;
+    if (prof) {
+      if (prof->mark(stream)) return -1;
+      prof->kind.push_back(KIND_EW);
+      prof->flops.push_back(0.0);
+    }
+  } else if (ctx.out_mask) {
     if (lr32 ? launch_upsample2x_argmax(lr32, ctx.out_mask, B, ctx.K, h2, w2, stream)
              : launch_upsample2x_argmax(lr, ctx.out_mask, B, ctx.K, h2, w2, stream))
       return -1;
@@ -1162,6 +1173,33 @@ int lseg_forward_argmax(lseg_engine* e, const float* x, int B, int H, int W, con
   ctx.out = logits;  // optional
   ctx.out_mask = mask;
   ctx.out_lr = nullptr;
+  return run_forward(e, ctx, B, H, W, static_cast<cudaStream_t>(stream));
+}
+
+int lseg_forward_segstats(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
+                          long long text_image_stride, const long long* target, const int* group, int nclass, int G,
+                          long long* stats, long long* mask, float* logits, void* stream) {
+  using namespace lseg;
+  SegStatsArgs st{target, group, stats, nclass, G};
+  if (!e || !text) {
+    set_error("lseg_forward_segstats: null %s", e ? "text" : "engine");
+    return -1;
+  }
+  // everything the output stage would reject is checked here, before the forward enqueues its first kernel
+  if (seg_stats_check("lseg_forward_segstats", x, st, B, H, W)) return -1;
+  if (H % 32 != 0 || W % 32 != 0 || W > 2 * kUpMaxW || K <= 0) {
+    set_error("lseg_forward_segstats: needs H, W multiples of 32, W <= %d, K > 0 (H=%d W=%d K=%d)", 2 * kUpMaxW, H, W, K);
+    return -1;
+  }
+  CallCtx ctx;
+  ctx.x = x;
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = K;
+  ctx.text_image_stride = text_image_stride;
+  ctx.out = logits;  // optional
+  ctx.out_mask = mask;  // optional
+  ctx.out_lr = nullptr;
+  ctx.seg = &st;
   return run_forward(e, ctx, B, H, W, static_cast<cudaStream_t>(stream));
 }
 

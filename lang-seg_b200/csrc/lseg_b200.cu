@@ -165,11 +165,18 @@ static int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* ba
   return 0;
 }
 
+// A barrier timeout (g_watchdog) is reported first; a bad metric group id (g_segstats_error, tag kSegStatsTag) when no
+// timeout is pending. Only the reported record is cleared, so a second call returns the other one.
 int read_watchdog(int out[4], cudaStream_t stream) {
   LSEG_CHECK_CUDA(cudaStreamSynchronize(stream));
   LSEG_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_watchdog, sizeof(int) * 4));
   int zero[4] = {0, 0, 0, 0};
-  LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_watchdog, zero, sizeof(zero)));
+  if (out[0] != 0) {
+    LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_watchdog, zero, sizeof(zero)));
+    return 0;
+  }
+  LSEG_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_segstats_error, sizeof(int) * 4));
+  if (out[0] != 0) LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_segstats_error, zero, sizeof(zero)));
   return 0;
 }
 
@@ -945,6 +952,20 @@ int lseg_head_block(const void* x, int in_f16, float* cmax_ws, float* y, int B, 
 int lseg_upsample2x_argmax(const void* lr, long long* mask, int B, int K, int H, int W, void* stream) {
   if (ensure_init()) return -1;
   return launch_upsample2x_argmax(static_cast<const __half*>(lr), mask, B, K, H, W, static_cast<cudaStream_t>(stream));
+}
+
+int lseg_seg_stats_scores(const float* scores, const long long* target, const int* group, int B, int K, int H, int W,
+                          int nclass, int G, long long* stats, void* stream) {
+  if (ensure_init()) return -1;
+  return launch_seg_stats_scores(scores, B, K, H, W, SegStatsArgs{target, group, stats, nclass, G},
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int lseg_seg_stats_mask(const long long* pred, const long long* target, const int* group, int B, int H, int W, int nclass,
+                        int G, long long* stats, void* stream) {
+  if (ensure_init()) return -1;
+  return launch_seg_stats_mask(pred, B, H, W, SegStatsArgs{target, group, stats, nclass, G},
+                               static_cast<cudaStream_t>(stream));
 }
 
 int lseg_text_embed(const int64_t* tokens, const float* tok_emb, const float* pos_emb, void* x, int K, int L, int Wd,

@@ -118,6 +118,35 @@ class Engine:
                                                     C.c_void_p(out.data_ptr()), lp, _stream()))
         return out
 
+    def forward_stats(self, x, text, k, target, stats, nclass, group=None, text_image_stride=0, mask=None, logits=None):
+        """Forward + argmax + metric counters in one output kernel: adds the counters of torch.max(logits, 1)[1] against
+        target int64 [B,H,W] to stats int64 [G, 3*nclass+2] (include/lseg_b200.h), in row group[b] for image b (row 0
+        without a group). Writes the mask / logits only into the tensors passed; enqueues on the current stream and does
+        not synchronise."""
+        from .ops import _check_stats, _group_ptr
+        self._check_input(x)
+        x = x.contiguous()
+        b, _, h, w = x.shape
+        _check_stats(stats, nclass)
+        if target.device != self.device or target.dtype != torch.int64 or tuple(target.shape) != (b, h, w):
+            raise ValueError(f"target must be int64 [B,H,W] = {(b, h, w)} on {self.device}")
+        if stats.device != self.device or not stats.is_contiguous():
+            raise ValueError(f"stats must be a contiguous tensor on {self.device}")
+        for name, t, dt, shape in (("mask", mask, torch.int64, (b, h, w)), ("logits", logits, torch.float32, (b, k, h, w))):
+            if t is not None and (t.device != self.device or t.dtype != dt or tuple(t.shape) != shape or
+                                  not t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous {dt} {shape} tensor on {self.device}")
+        target = target.contiguous()
+        g, gp = _group_ptr(group, stats, b)
+        mp = C.c_void_p(mask.data_ptr()) if mask is not None else None
+        lp = C.c_void_p(logits.data_ptr()) if logits is not None else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_forward_segstats(self.handle, C.c_void_p(x.data_ptr()), b, h, w,
+                                                      C.c_void_p(text.data_ptr()), k, text_image_stride,
+                                                      C.c_void_p(target.data_ptr()), gp, nclass, stats.shape[0],
+                                                      C.c_void_p(stats.data_ptr()), mp, lp, _stream()))
+        return stats
+
     def forward_profiled(self, x, text, k, text_image_stride=0, out=None):
         """One forward with CUDA events around every launch. Returns (out, [(ms, kind, flops), ...])."""
         x = x.contiguous()

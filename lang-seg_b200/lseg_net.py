@@ -367,21 +367,37 @@ class LSegNet(_LSegBase):
             raise ValueError("out must be a contiguous float32 [B,K,H,W] tensor")
         return engine.forward(x.float(), feats, text.shape[0], out=out)
 
+    def _labelset_tokens(self, labelset):
+        if isinstance(labelset, torch.Tensor):
+            return labelset
+        if isinstance(labelset, str) and labelset == "":
+            return self.text
+        return tokenize(labelset)
+
     @torch.no_grad()
     def predict(self, x, labelset=""):
         """torch.max(self.forward(x, labelset), 1)[1] — what every caller of the reference does with the logits
         (lseg_app.py:357-360, test_lseg.py:397) — fused on the device: int64 [B,H,W], the fp32 [B,K,H,W] logits are
         never written (SURVEY.md 8(f) row 2)."""
         self._check_eval()
-        if isinstance(labelset, torch.Tensor):
-            text = labelset
-        elif isinstance(labelset, str) and labelset == "":
-            text = self.text
-        else:
-            text = tokenize(labelset)
+        text = self._labelset_tokens(labelset)
         engine = self._engine_for(x.device)
         feats = self._text_features(engine, text)
         return engine.forward_argmax(x.float(), feats, text.shape[0])
+
+    @torch.no_grad()
+    def update_metric(self, metric, x, target, labelset=""):
+        """metric.update(target, self.forward(x, labelset)) for a lseg_b200.metrics.SegmentationMetric, fused into the
+        output kernel: the counters of torch.max(logits, 1)[1] against target (int64 [B,H,W], or [H,W] for B = 1; -1 =
+        ignored) are added on the device. Neither logits nor mask are written, and nothing synchronises."""
+        from .metrics import _as_target
+        self._check_eval()
+        text = self._labelset_tokens(labelset)
+        engine = self._engine_for(x.device)
+        feats = self._text_features(engine, text)
+        stats = metric._buffer(x.device)
+        t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
+        engine.forward_stats(x.float(), feats, text.shape[0], t, stats, metric.nclass)
 
 
 class LSegNetZS(_LSegBase):
@@ -440,6 +456,21 @@ class LSegNetZS(_LSegBase):
         self._check_eval()
         engine = self._engine_for(x.device)
         return engine.forward_argmax(x.float(), self._image_text(engine, class_info, x.device), 2, text_image_stride=2)
+
+    @torch.no_grad()
+    def update_metric(self, meter, x, class_info, target, query_ignore_idx=None):
+        """Evaluator.classify_prediction(self.predict(x, class_info), target, query_ignore_idx) followed by
+        meter.update(..., class_info) for a lseg_b200.metrics.FewShotMeter, fused into the output kernel: image b's
+        counters go straight to the meter's row class_info[b]. Neither logits nor mask are written; the one host
+        synchronisation is forward()'s class_info range check. A padded input takes a target padded with -1."""
+        from .metrics import _as_target, _fewshot_target
+        self._check_eval()
+        engine = self._engine_for(x.device)
+        text = self._image_text(engine, class_info, x.device)
+        t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
+        t = _fewshot_target(t, query_ignore_idx)
+        group = torch.as_tensor(class_info).to(x.device)
+        engine.forward_stats(x.float(), text, 2, t, meter.stats, 2, group=group, text_image_stride=2)
 
 
 class LSegRNNetZS(LSegNetZS):

@@ -298,6 +298,50 @@ def upsample2x_argmax(x):
     return m
 
 
+def _group_ptr(group, stats, B):
+    """int32 device copy of a group-id tensor of B entries (None: every image counts into row 0). Values outside int32
+    are clamped into it, where they stay out of [0, G), so the device check still reports them."""
+    if group is None:
+        return None, None
+    group = torch.as_tensor(group)
+    if group.numel() != B:
+        raise ValueError(f"group has {group.numel()} entries, the batch has {B} images")
+    g = group.reshape(-1).to(device=stats.device, dtype=torch.int64).clamp(-2 ** 31, 2 ** 31 - 1).to(torch.int32)
+    g = g.contiguous()
+    return g, _ptr(g)
+
+
+def _check_stats(stats, nclass):
+    if stats.dtype != torch.int64 or stats.dim() != 2 or stats.shape[1] != 3 * nclass + 2:
+        raise ValueError(f"stats must be int64 [G, 3*nclass+2] = [G, {3 * nclass + 2}], got {stats.dtype} "
+                         f"{tuple(stats.shape)}")
+
+
+def seg_stats_scores(scores, target, stats, nclass, group=None):
+    """Adds the metric counters of fp32 scores [B,K,H,W] (first maximal class) against int64 target [B,H,W] to
+    stats int64 [G, 3*nclass+2] (row layout and per-pixel rule: include/lseg_b200.h). group: ids [B] or None."""
+    B, K, H, W = scores.shape
+    _check_stats(stats, nclass)
+    if tuple(target.shape) != (B, H, W):
+        raise ValueError(f"target must be [B,H,W] = {(B, H, W)}, got {tuple(target.shape)}")
+    g, gp = _group_ptr(group, stats, B)
+    check(load().lseg_seg_stats_scores(_ptr(scores, torch.float32), _ptr(target, torch.int64), gp, B, K, H, W, nclass,
+                                       stats.shape[0], _ptr(stats, torch.int64), _stream()))
+    return stats
+
+
+def seg_stats_mask(pred, target, stats, nclass, group=None):
+    """Adds the metric counters of an int64 prediction mask [B,H,W] against int64 target [B,H,W] to stats."""
+    B, H, W = pred.shape
+    _check_stats(stats, nclass)
+    if tuple(target.shape) != (B, H, W):
+        raise ValueError(f"target must be [B,H,W] = {(B, H, W)}, got {tuple(target.shape)}")
+    g, gp = _group_ptr(group, stats, B)
+    check(load().lseg_seg_stats_mask(_ptr(pred, torch.int64), _ptr(target, torch.int64), gp, B, H, W, nclass,
+                                     stats.shape[0], _ptr(stats, torch.int64), _stream()))
+    return stats
+
+
 def text_embed(tokens, tok_emb, pos_emb):
     K, L = tokens.shape
     Wd = tok_emb.shape[1]

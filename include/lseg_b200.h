@@ -97,6 +97,15 @@ int lseg_gemm(const lseg_gemm_args* args, void* stream);
  *   out[4] kernel instantiation: 0 register-direct, 1 TMA fp16, 2 TMA reduce-add, 3 fixed split-K, 4 grouped NCHW store
  *          (nchw_group > 0), 5 ReLU after the fp32 residual. */
 int lseg_debug_gemm_plan(const lseg_gemm_args* args, int out[5]);
+/* Debug: for the same plan, out[0] = its cluster size (1, or 2: pairs of CTAs computing n-tiles 2j and 2j+1 of one m-tile,
+ * each loading half of the shared A tile for both) and out[1] = the number of clusters it launches (out[1] * out[0] =
+ * lseg_debug_gemm_plan's grid). Pairs are possible when the n-tile count is even and tiles are not split stream-K; the
+ * planner uses them when the plan has more work units (tiles, or tiles x fixed split-K segments) than the device has SMs. */
+int lseg_debug_gemm_cluster(const lseg_gemm_args* args, int out[2]);
+/* Debug: how GEMMs planned after this call choose their cluster size: 1 = never pair CTAs, 2 = the planner's rule
+ * (default), 3 = pair CTAs in every plan where that is possible. Results are bit-identical in all three modes. Any other
+ * value is rejected. */
+int lseg_debug_set_gemm_cluster(int mode);
 
 /* Fused MHSA, head_dim 64 (k5; timm Attention restated at lseg_vit.py:26-39; CLIP text MHA).
  * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64].
@@ -119,8 +128,9 @@ int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* st
  * 0 (or LSEG_SPLITK=1): an in-place fp32 residual GEMM without an activation (the MLP's fc2) may split a tile's K range
  * over two CTAs whose partial sums are reduce-added in arrival order (differences at the fp32 rounding level, hence off by default). */
 int lseg_set_deterministic(int on);
-/* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTAs
- * into trace ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). Row w of a CTA is
+/* Debug: GEMMs planned after this call stamp clock64() at the epilogue / MMA hand-off points of two CTAs, blockIdx.x 0
+ * and gridDim.x / 2 (in a clustered plan, rank 0 of their pair when the cluster count is even), into trace
+ * ([2][20 warps][512] uint64 device memory, zeroed by the caller; NULL switches it off). Row w of a CTA is
  * warp w: rows 4-7 are consumer warpgroup 0 and rows 8-11 warpgroup 1, each stamping only the tiles it owns (every
  * other entry of the CTA's work list); the other rows stay zero. Stamp = clock64() << 8 | tag. */
 int lseg_debug_gemm_trace(unsigned long long* trace);

@@ -38,6 +38,18 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// Arrival on the mbarrier at the same shared-memory offset in CTA `rank` of this thread's cluster. Relaxed: it orders
+// nothing, so the caller must have COMPLETED (not merely issued) whatever the arrival hands over — e.g. wgmma_wait
+// before releasing an operand stage. (Measured on an H100 80GB HBM3 at 700 W: with .release.cluster arrivals, one per
+// consumer warp and k-chunk, the clustered QKV GEMM took 2.1x the unclustered time; relaxed, 1.06x.)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(rank)
+      : "memory");
+}
 // suspend-time hint: the waiting thread sleeps in hardware until the phase completes or this many ns
 // pass, instead of re-polling every ~100 cycles and stealing issue slots from the compute warps that
 // share its SM sub-partition.
@@ -172,6 +184,28 @@ __device__ __forceinline__ bool elect_one_sync() {
 }
 __device__ __forceinline__ int warp_idx_sync() { return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0); }
 
+// ---- thread block clusters ------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t num_clusters_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+  return r;
+}
+// Every thread of every CTA of the cluster: shared-memory writes and mbarrier operations before it (release) are
+// visible to all of the cluster's threads after it (acquire). Not .aligned: callers may be diverged within a warp.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+
 // Per-warpgroup register budget (all 128 threads of the warpgroup execute it): a warpgroup that only issues TMA hands
 // registers back to the pool, and the MMA warpgroups claim them. The budgets of all warpgroups must fit the CTA's
 // allocation at launch (registers per thread from ptxas x threads).
@@ -220,6 +254,24 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
       "[%2];" ::"r"(smem_u32(dst)),
       "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+// Multicast forms: the box lands at the same shared-memory offset in every CTA of the cluster named in cta_mask, and
+// each of them credits its bytes to the mbarrier at bar's offset in that CTA.
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      int c2, int c3, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
+      "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(cta_mask)
       : "memory");
 }
 
@@ -404,21 +456,36 @@ const char* get_error();
   } while (0)
 
 // Kernel launch with the PDL attribute (see griddep_wait above); LSEG_NO_PDL=1 falls back to plain launches.
+// cluster > 1: grid.x CTAs in clusters of `cluster` along x (grid.x a multiple of it).
 template <typename... KArgs, typename... Args>
-static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                                     Args&&... args) {
+static inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, int cluster,
+                                             cudaStream_t stream, Args&&... args) {
   static const bool no_pdl = getenv("LSEG_NO_PDL") != nullptr;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  if (!no_pdl) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cluster > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = cluster;
+    attr[n].val.clusterDim.y = 1;
+    attr[n++].val.clusterDim.z = 1;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = no_pdl ? 0 : 1;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                     Args&&... args) {
+  return launch_pdl_cluster(kernel, grid, block, smem, 1, stream, static_cast<Args&&>(args)...);
 }
 
 // Encode a tiled fp16 tensor map (rank 2..4), 128-byte swizzle, zero OOB fill.

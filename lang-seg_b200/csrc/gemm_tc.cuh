@@ -18,8 +18,10 @@
 // runs while the other's MMAs keep the tensor cores busy; the tensor pipe idles only where an epilogue takes longer
 // than a main loop, or where a CTA owns a single tile. The accumulation order of every output element (the same
 // k16 chunks through the same m64n128k16 instruction) does not depend on which warpgroup computes the tile.
-// Measured (B=8, 480x480, H100 80GB HBM3 SXM at a 700 W power limit, tools/gemm_shapes.py): ViT linears 460-530
-// TFLOP/s (QKV, fc1) and 320-410 (proj, fc2); 3x3 decoder convs 310-440 at 60^2 / 120^2.
+// Grids with more work units than SMs and an even n-tile count run as 2-CTA clusters that share the A tile (CLUSTER,
+// see the kernel); lseg_b200.cu (gemm_plan_grid) has the rule and the numbers behind it.
+// Measured (B=8, 480x480, H100 80GB HBM3 SXM at a 700 W power limit, tools/gemm_shapes.py, as planned): ViT linears
+// 480-510 TFLOP/s (QKV, fc1) and 340-400 (proj, fc2); 3x3 decoder convs 320-480 at 60^2 / 120^2; head1 280.
 //
 // Epilogue modes:
 //   EPI_DIRECT   stores straight from registers, thread <-> accumulator row.
@@ -565,7 +567,17 @@ __device__ __forceinline__ void gemm_stage_half(float* acc_half, float (&acc)[64
 
 // FIXED_SPLIT: the deterministic split-K schedule (GemmParams::split_fixed) is its own instantiation, so its index
 // arithmetic stays out of the other kernels.
-template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false>
+// CLUSTER: the grid is made of 2-CTA clusters, and both CTAs of a cluster walk the same work list of pair units
+// (m_tile, n_pair) — (m_tile, n_pair, segment) under FIXED_SPLIT — in the m-fastest order of the unclustered list; the CTA
+// of rank r computes n-tile 2 n_pair + r. The A tile is the same for both, so rank r loads only its rows 64 r .. 64 r + 63
+// (the A tensor map's box is half a tile: {64, 64}, or {64, 16, 4, 1} = pixel rows 4 r .. 4 r + 3 of a conv tile) and
+// multicasts them to the same ring offset in both CTAs; B stays per CTA. Each full barrier still expects the whole stage
+// (16 KB of A, half from each rank, + 16 KB of B). Since either producer writes a stage of both CTAs, a stage is free only
+// once the on-turn consumer warps of both CTAs have released it: every consumer warp arrives on the empty barrier of its
+// own CTA and on the peer's (count 8). The two lists have the same k ranges, so the ring stage / parity sequence and the
+// ping-pong turn order are the same in both CTAs. Every output element sums the same k16 chunks in the same order through
+// the same instruction as without clusters: results are bit-identical. Needs an even n-tile count and no stream-K split.
+template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false, bool CLUSTER = false>
 __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   static_assert(!RELU_RES || (EPI == EPI_DIRECT && !FIXED_SPLIT && !GROUPED), "relu-after-residual: plain register-direct");
   static_assert(!FIXED_SPLIT || EPI == EPI_DIRECT, "split-K partials leave through the register-direct epilogue");
@@ -581,8 +593,10 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
 
   const int warp = warp_idx_sync();  // provably warp-uniform: role branches and their operands stay on the uniform datapath
   const int lane = threadIdx.x & 31;
-  const int cta = blockIdx.x;
-  const int num_ctas = gridDim.x;
+  // work list index and count: one list per CTA, or per cluster
+  const int cta = CLUSTER ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
+  const int num_ctas = CLUSTER ? static_cast<int>(num_clusters_x()) : static_cast<int>(gridDim.x);
+  const int rank = CLUSTER ? static_cast<int>(cluster_ctarank()) : 0;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tma_a);
@@ -590,15 +604,19 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     if (EPI != EPI_DIRECT) tma_prefetch_desc(&p.tma_c);
     for (int i = 0; i < Cfg::kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 4);
+      mbar_init(&empty_bar[i], CLUSTER ? 8 : 4);
     }
     mbar_fence_init();
   }
   griddep_launch_dependents();
-  __syncthreads();
+  if constexpr (CLUSTER)
+    cluster_sync();  // the peer's barriers are initialised before its first multicast or remote arrival reaches them
+  else
+    __syncthreads();
   griddep_wait();  // everything above overlapped the previous kernel's tail; operands / outputs are touched below
 
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  // CLUSTER: the list is over pair units (num_n_tiles is even)
+  const int num_tiles = p.num_m_tiles * (CLUSTER ? p.num_n_tiles / 2 : p.num_n_tiles);
 
   // Work schedule of this CTA. Default: whole tiles cta, cta + G, ... . split_k (in-place residual GEMMs only, whose
   // epilogue is a reduce-add and therefore composes over partial sums): the (tile, k-chunk) units are dealt out evenly,
@@ -641,7 +659,7 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     sc.tile_step = num_ctas;
     sc.num_tiles = num_tiles;
     sc.k_iters = p.k_iters;
-    sc.split = (EPI == EPI_TMA_ADD) && p.split_k;
+    sc.split = (EPI == EPI_TMA_ADD) && !CLUSTER && p.split_k;
     sc.fixed = FIXED_SPLIT ? p.split_fixed : 0;
     sc.seg = 0;
     const long long units = static_cast<long long>(num_tiles) * p.k_iters;
@@ -654,16 +672,17 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
 
   if (warp < 4) {
     // ===================== TMA producer warpgroup: warp 0 issues, warps 1-3 only hand their registers back =====================
+    // (CLUSTER: warps 1-3 stay until the final cluster barrier instead of exiting)
     setmaxnreg_dec<Cfg::kProducerRegs>();
-    if (warp != 0) return;
+    if (!CLUSTER && warp != 0) return;
     const bool leader = elect_one_sync();  // converged warp, elected issuing lane
     int stage = 0;
     uint32_t phase = 0;
     Sched sc = make_sched();
     int tile, k_begin, k_end;
-    while (sc.next(tile, k_begin, k_end)) {
+    while ((!CLUSTER || warp == 0) && sc.next(tile, k_begin, k_end)) {
       const int m_tile = tile % p.num_m_tiles;
-      const int n0 = (tile / p.num_m_tiles) * kGemmBN;
+      const int n0 = (CLUSTER ? 2 * (tile / p.num_m_tiles) + rank : tile / p.num_m_tiles) * kGemmBN;
       int cb = 0, ch0 = 0, cw0 = 0;
       if (p.conv) {
         const int per_img = p.tiles_h * p.tiles_w;
@@ -694,10 +713,18 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
         }
         if (leader) {
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          if (p.conv)
-            tma_load_4d(sa, &p.tma_a, &full_bar[stage], c0, c1, c2, cb);
-          else
-            tma_load_2d(sa, &p.tma_a, &full_bar[stage], c0, c1);
+          if constexpr (CLUSTER) {  // this rank's half of the A tile, into both CTAs
+            uint8_t* sa_half = sa + rank * (Cfg::kABytes / 2);
+            if (p.conv)
+              tma_load_4d_multicast(sa_half, &p.tma_a, &full_bar[stage], c0, c1, c2 + rank * (kConvTH / 2), cb, 0x3);
+            else
+              tma_load_2d_multicast(sa_half, &p.tma_a, &full_bar[stage], c0, c1 + rank * (kGemmBM / 2), 0x3);
+          } else {
+            if (p.conv)
+              tma_load_4d(sa, &p.tma_a, &full_bar[stage], c0, c1, c2, cb);
+            else
+              tma_load_2d(sa, &p.tma_a, &full_bar[stage], c0, c1);
+          }
           tma_load_2d(sb, &p.tma_b, &full_bar[stage], kit * kGemmBK, n0);
         }
         __syncwarp();
@@ -723,7 +750,8 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     int stage = 0;
     uint32_t phase = 0;
     GemmTrace tr;
-    if (p.trace && lane == 0 && (cta == 0 || cta == num_ctas / 2)) tr.w = p.trace + ((cta == 0 ? 0 : 1) * 20 + warp) * 512;
+    const int bid = blockIdx.x;  // traced: CTAs 0 and gridDim.x / 2 (clustered plans: both are rank 0 of their pair)
+    if (p.trace && lane == 0 && (bid == 0 || bid == static_cast<int>(gridDim.x) / 2)) tr.w = p.trace + ((bid == 0 ? 0 : 1) * 20 + warp) * 512;
     tr(0);
     float acc0[64], acc1[64];
 #pragma unroll
@@ -733,7 +761,7 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     bool more = sc.next(tile, k_begin, k_end);
     for (int idx = 0; more; ++idx) {
       const int m_tile = tile % p.num_m_tiles;
-      const int n_tile = tile / p.num_m_tiles;
+      const int n_tile = CLUSTER ? 2 * (tile / p.num_m_tiles) + rank : tile / p.num_m_tiles;
       const int kb = k_begin, ke = k_end;
       const int seg = FIXED_SPLIT ? sc.seg : 0;
       more = sc.next(tile, k_begin, k_end);  // entry idx + 1
@@ -761,8 +789,11 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
           }
           wgmma_commit();
         }
-        wgmma_wait<1>();  // the previous chunk's MMAs have read their stage: hand it back to the producer
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        wgmma_wait<1>();  // the previous chunk's MMAs have read their stage (complete): hand it back to the producer(s)
+        if (prev >= 0 && lane == 0) {
+          mbar_arrive(&empty_bar[prev]);
+          if constexpr (CLUSTER) mbar_arrive_cluster(&empty_bar[prev], rank ^ 1);
+        }
         prev = stage;
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
@@ -770,7 +801,10 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
       wgmma_wait<0>();
       wgmma_reg_fence(acc0);
       wgmma_reg_fence(acc1);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0 && lane == 0) {
+        mbar_arrive(&empty_bar[prev]);
+        if constexpr (CLUSTER) mbar_arrive_cluster(&empty_bar[prev], rank ^ 1);
+      }
       tr(12);
       // Epilogue, one column half at a time through this warpgroup's staging area. Barrier 3 + wg: no warp of the
       // warpgroup still reads the area (previous half or tile) when it is rewritten, and all of it is written before
@@ -791,6 +825,9 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     }
     if (EPI != EPI_DIRECT && elect_one_sync()) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem
   }
+  // CLUSTER: no CTA leaves while its peer may still arrive on its barriers (the peer's consumers release their last
+  // stages on both CTAs)
+  if constexpr (CLUSTER) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------

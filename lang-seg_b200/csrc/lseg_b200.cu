@@ -45,6 +45,11 @@ static int g_plan_epoch = 0;     // bumped when an option that is baked into cac
 static unsigned long long* g_gemm_trace = nullptr;  // debug (lseg_debug_gemm_trace)
 static int g_gemm_probe = 0;
 static int g_mhsa_variant = 0;   // kernel the engine's ViT attention runs (lseg_mhsa_variant documents the numbering)
+static int g_gemm_cluster_mode = 2;  // lseg_debug_set_gemm_cluster: 1 never, 2 the planner's rule, 3 wherever allowed
+// Which gemm_tc_kernel instantiation runs a plan (numbering of lseg_debug_gemm_plan's out[4]).
+enum GemmKernel { GK_DIRECT = 0, GK_TMA_F16 = 1, GK_TMA_ADD = 2, GK_FIXED_SPLIT = 3, GK_GROUPED_NCHW = 4, GK_RELU_RES = 5,
+                  GK_COUNT = 6 };
+static int g_gemm_active_pairs[GK_COUNT];  // per instantiation: 2-CTA clusters of it that fit on the device at once
 static std::mutex g_init_mutex;
 static bool g_global_init = false;
 constexpr int kMaxDevices = 64;
@@ -67,6 +72,30 @@ static int init_global() {
   return 0;
 }
 
+// Opt-in shared memory of both forms of one gemm_tc_kernel instantiation, and how many 2-CTA clusters of the clustered
+// form the device holds at once (not simply SMs / 2: a cluster's CTAs share one GPC, and a GPC may have an odd SM count).
+template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false>
+static int gemm_init_kernel(int* active_pairs) {
+  auto plain = gemm_tc_kernel<EPI, FIXED_SPLIT, GROUPED, RELU_RES, false>;
+  auto paired = gemm_tc_kernel<EPI, FIXED_SPLIT, GROUPED, RELU_RES, true>;
+  const int smem = GemmCfg<EPI>::kSmemBytes;
+  if (cudaFuncSetAttribute(plain, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||
+      cudaFuncSetAttribute(paired, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+    return -1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2);
+  cfg.blockDim = dim3(GemmCfg<EPI>::kThreads);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  return cudaOccupancyMaxActiveClusters(active_pairs, paired, &cfg) == cudaSuccess ? 0 : -1;
+}
+
 // Per-device part: architecture check and the function attributes (opt-in shared memory sizes are a property of
 // (function, device); a process that drives several GPUs — DataParallel replicas, additional_utils/models.py:183-248 —
 // must set them on each one).
@@ -87,15 +116,16 @@ static int init_device(int dev) {
     return -1;
   }
   g_num_sms = prop.multiProcessorCount;
-#define LSEG_SET_SMEM(KERNEL, EPI_) \
-  cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<EPI_>::kSmemBytes)
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT>), EPI_DIRECT);
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_TMA_F16>), EPI_TMA_F16);
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_TMA_ADD>), EPI_TMA_ADD);
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT);
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT);
-  LSEG_SET_SMEM((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT);
-#undef LSEG_SET_SMEM
+  int pairs[GK_COUNT];
+  if (gemm_init_kernel<EPI_DIRECT>(&pairs[GK_DIRECT]) || gemm_init_kernel<EPI_TMA_F16>(&pairs[GK_TMA_F16]) ||
+      gemm_init_kernel<EPI_TMA_ADD>(&pairs[GK_TMA_ADD]) ||
+      gemm_init_kernel<EPI_DIRECT, true>(&pairs[GK_FIXED_SPLIT]) ||
+      gemm_init_kernel<EPI_DIRECT, false, true>(&pairs[GK_GROUPED_NCHW]) ||
+      gemm_init_kernel<EPI_DIRECT, false, false, true>(&pairs[GK_RELU_RES])) {
+    set_error("lseg_b200: GEMM kernel attributes / cluster occupancy query failed on device %d", dev);
+    return -1;
+  }
+  memcpy(g_gemm_active_pairs, pairs, sizeof(pairs));
   cudaFuncSetAttribute(mhsa_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   cudaFuncSetAttribute(mhsa_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   cudaFuncSetAttribute(mhsa_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
@@ -185,7 +215,8 @@ int read_watchdog(int out[4], cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 struct GemmPlan {
   GemmParams p;
-  int grid;
+  int grid;     // CTAs
+  int cluster;  // 1, or 2: CTA pairs that share the A tile (gemm_tc_kernel CLUSTER); grid is then even
   int epi;      // GemmEpiMode
   // deterministic split-K (gemm_tc.cuh splitk_reduce_kernel): p.split_fixed segments per tile write raw partials to a
   // workspace the CALLER provides (gemm_set_workspace) before gemm_run; final_epi is the epilogue the reduce applies
@@ -220,6 +251,41 @@ static int gemm_pick_split(const GemmDesc& d, const GemmParams& p, int n_tiles, 
 }
 
 static void gemm_set_workspace(GemmPlan* plan, float* ws) { plan->p.e.out_f32 = ws; }
+
+static int gemm_kernel_of(const GemmPlan& plan);
+// Last step of gemm_plan: cluster size, grid, and the A tensor map, whose box is what one CTA loads (a whole 128-row
+// tile, or the half a CTA of a pair multicasts). Pairs need an even n-tile count (no dummy tiles) and whole tiles per work
+// unit (stream-K ranges are per CTA). The units are tiles, or tiles x segments under the fixed split-K schedule.
+// The planner pairs CTAs only when there are more work units than SMs. Measured with tools/gemm_shapes.py (B = 8, 480^2,
+// H100 80GB HBM3 at 700 W, paired vs unclustered, two runs): with several units per CTA, pairs were faster on the ViT
+// proj / fc1 / fc2 (+4 to +8 %), the 120^2 and 60^2 3x3 convs (+4 to +18 %), the 120^2 1x1 out_conv (+12 %), head1
+// (+40 %; its 236 MB A operand exceeds L2, and a pair fetches each A tile once for two n-tiles) and pixel x text
+// (+5 %); QKV was within 1 % (-0.6 / -1.0 %). Where every CTA owns at most one unit (the 30^2 convs: 128 tiles; the
+// 15^2 split-K convs: 128 units) pairs only add their barrier round trips: layer_rn and RCU conv2 at 30^2 and 15^2 were
+// 0.4 to 3.2 % slower in both runs, RCU conv1 +4 % to -11 %.
+static int gemm_plan_grid(const GemmDesc& d, GemmPlan* plan) {
+  GemmParams& p = plan->p;
+  const int pairs = g_gemm_active_pairs[gemm_kernel_of(*plan)];
+  const int units = p.num_m_tiles * p.num_n_tiles * (p.split_fixed > 1 ? p.split_fixed : 1);
+  const bool allowed = p.num_n_tiles % 2 == 0 && !p.split_k && pairs > 0;
+  const bool wanted = g_gemm_cluster_mode == 3 || (g_gemm_cluster_mode == 2 && units > g_num_sms);
+  plan->cluster = (allowed && wanted) ? 2 : 1;
+  if (plan->cluster == 2)
+    plan->grid = 2 * (units / 2 < pairs ? units / 2 : pairs);
+  else
+    plan->grid = units < g_num_sms ? units : g_num_sms;
+  const int rows = kGemmBM / plan->cluster;
+  if (d.conv) {
+    const uint64_t dims[4] = {(uint64_t)d.K, (uint64_t)d.W, (uint64_t)d.H, (uint64_t)d.B};
+    const uint64_t str[3] = {(uint64_t)d.K * 2, (uint64_t)d.K * d.W * 2, (uint64_t)d.K * d.W * d.H * 2};
+    const uint32_t box[4] = {kGemmBK, kConvTW, (uint32_t)rows / kConvTW, 1};
+    return make_tmap_f16(&p.tma_a, d.a, 4, dims, str, box);
+  }
+  const uint64_t dims[2] = {(uint64_t)d.K, (uint64_t)d.a_rows};
+  const uint64_t str[1] = {(uint64_t)d.lda * 2};
+  const uint32_t box[2] = {kGemmBK, (uint32_t)rows};
+  return make_tmap_f16(&p.tma_a, d.a, 2, dims, str, box);
+}
 
 static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
   if (ensure_init()) return -1;
@@ -267,16 +333,8 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     p.tiles_h = (d.H + kConvTH - 1) / kConvTH;
     p.tiles_w = (d.W + kConvTW - 1) / kConvTW;
     p.num_m_tiles = d.B * p.tiles_h * p.tiles_w;
-    const uint64_t dims[4] = {(uint64_t)d.K, (uint64_t)d.W, (uint64_t)d.H, (uint64_t)d.B};
-    const uint64_t str[3] = {(uint64_t)d.K * 2, (uint64_t)d.K * d.W * 2, (uint64_t)d.K * d.W * d.H * 2};
-    const uint32_t box[4] = {kGemmBK, kConvTW, kConvTH, 1};
-    if (make_tmap_f16(&p.tma_a, d.a, 4, dims, str, box)) return -1;
   } else {
     p.num_m_tiles = (d.M + kGemmBM - 1) / kGemmBM;
-    const uint64_t dims[2] = {(uint64_t)d.K, (uint64_t)d.a_rows};
-    const uint64_t str[1] = {(uint64_t)d.lda * 2};
-    const uint32_t box[2] = {kGemmBK, kGemmBM};
-    if (make_tmap_f16(&p.tma_a, d.a, 2, dims, str, box)) return -1;
   }
   p.num_n_tiles = (d.N + kGemmBN - 1) / kGemmBN;
   {
@@ -302,13 +360,11 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
       p.e.ldc = d.N;
       p.e.row_scale = 1.f;
       plan->ws_bytes = sizeof(float) * static_cast<size_t>(split) * d.M * d.N;
-      const int units = tiles * split;
-      plan->grid = units < g_num_sms ? units : g_num_sms;
       if (d.e.store == STORE_ROWMAJOR && (d.e.ldc % 8 != 0)) {
         set_error("gemm: ldc must be a multiple of 8");
         return -1;
       }
-      return 0;
+      return gemm_plan_grid(d, plan);
     }
   }
   {
@@ -344,7 +400,6 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
                    p.k_iters >= min_kit) ? 1 : 0;
     }
   }
-  plan->grid = tiles < g_num_sms ? tiles : g_num_sms;
   if (p.e.store == STORE_D2S && (p.e.d2s_cout % 32 != 0 || !p.e.out_f16)) {
     set_error("gemm: depth-to-space store needs cout %% 32 == 0 and an fp16 output");
     return -1;
@@ -353,7 +408,7 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
     set_error("gemm: ldc must be a multiple of 8");
     return -1;
   }
-  return 0;
+  return gemm_plan_grid(d, plan);
 }
 
 static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream);
@@ -374,8 +429,6 @@ static int gemm_run(const GemmPlan& plan, cudaStream_t stream) {
   }
   return gemm_run_kernel(plan, stream);
 }
-// Which gemm_tc_kernel instantiation runs a plan (numbering of lseg_debug_gemm_plan's out[4]).
-enum GemmKernel { GK_DIRECT = 0, GK_TMA_F16 = 1, GK_TMA_ADD = 2, GK_FIXED_SPLIT = 3, GK_GROUPED_NCHW = 4, GK_RELU_RES = 5 };
 static int gemm_kernel_of(const GemmPlan& plan) {
   if (plan.epi == EPI_TMA_F16) return GK_TMA_F16;
   if (plan.epi == EPI_TMA_ADD) return GK_TMA_ADD;
@@ -384,18 +437,24 @@ static int gemm_kernel_of(const GemmPlan& plan) {
   if (plan.p.e.relu_after_res) return GK_RELU_RES;
   return GK_DIRECT;
 }
+template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false>
+static void gemm_launch(const GemmPlan& plan, cudaStream_t stream) {
+  const dim3 grid(plan.grid), block(GemmCfg<EPI>::kThreads);
+  if (plan.cluster == 2)
+    launch_pdl_cluster(gemm_tc_kernel<EPI, FIXED_SPLIT, GROUPED, RELU_RES, true>, grid, block, GemmCfg<EPI>::kSmemBytes,
+                       2, stream, plan.p);
+  else
+    launch_pdl(gemm_tc_kernel<EPI, FIXED_SPLIT, GROUPED, RELU_RES>, grid, block, GemmCfg<EPI>::kSmemBytes, stream, plan.p);
+}
 static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream) {
-#define LSEG_LAUNCH(KERNEL, EPI_) \
-  launch_pdl(KERNEL, dim3(plan.grid), dim3(GemmCfg<EPI_>::kThreads), GemmCfg<EPI_>::kSmemBytes, stream, plan.p)
   switch (gemm_kernel_of(plan)) {
-    case GK_TMA_F16: LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_F16>, EPI_TMA_F16); break;
-    case GK_TMA_ADD: LSEG_LAUNCH(gemm_tc_kernel<EPI_TMA_ADD>, EPI_TMA_ADD); break;
-    case GK_FIXED_SPLIT: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, true>), EPI_DIRECT); break;
-    case GK_GROUPED_NCHW: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, true>), EPI_DIRECT); break;
-    case GK_RELU_RES: LSEG_LAUNCH((gemm_tc_kernel<EPI_DIRECT, false, false, true>), EPI_DIRECT); break;
-    default: LSEG_LAUNCH(gemm_tc_kernel<EPI_DIRECT>, EPI_DIRECT); break;
+    case GK_TMA_F16: gemm_launch<EPI_TMA_F16>(plan, stream); break;
+    case GK_TMA_ADD: gemm_launch<EPI_TMA_ADD>(plan, stream); break;
+    case GK_FIXED_SPLIT: gemm_launch<EPI_DIRECT, true>(plan, stream); break;
+    case GK_GROUPED_NCHW: gemm_launch<EPI_DIRECT, false, true>(plan, stream); break;
+    case GK_RELU_RES: gemm_launch<EPI_DIRECT, false, false, true>(plan, stream); break;
+    default: gemm_launch<EPI_DIRECT>(plan, stream); break;
   }
-#undef LSEG_LAUNCH
   LSEG_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -778,6 +837,27 @@ int lseg_debug_gemm_plan(const lseg_gemm_args* a, int out[5]) {
   out[2] = plan.p.split_k;
   out[3] = plan.p.split_fixed;
   out[4] = gemm_kernel_of(plan);
+  return 0;
+}
+
+int lseg_debug_gemm_cluster(const lseg_gemm_args* a, int out[2]) {
+  GemmDesc d;
+  if (gemm_desc_of(a, d)) return -1;
+  GemmPlan plan;
+  if (gemm_plan(d, &plan)) return -1;
+  out[0] = plan.cluster;
+  out[1] = plan.grid / plan.cluster;
+  return 0;
+}
+
+int lseg_debug_set_gemm_cluster(int mode) {
+  if (mode < 1 || mode > 3) {
+    set_error("debug_set_gemm_cluster: mode must be 1, 2 or 3, got %d", mode);
+    return -1;
+  }
+  if (ensure_init()) return -1;
+  if (mode != g_gemm_cluster_mode) ++g_plan_epoch;
+  g_gemm_cluster_mode = mode;
   return 0;
 }
 

@@ -103,6 +103,20 @@ def gemm_plan(a, w, N=None, **kw):
     return dict(zip(("epi", "grid", "split_k", "split_fixed", "kernel"), out))
 
 
+def gemm_cluster(a, w, N=None, **kw):
+    """Cluster layout of the plan gemm(a, w, N, **kw) would run (include/lseg_b200.h lseg_debug_gemm_cluster):
+    dict with cluster (1, or 2 for CTA pairs sharing the A tile) and clusters (how many it launches)."""
+    out = (C.c_int * 2)()
+    check(load().lseg_debug_gemm_cluster(C.byref(_gemm_args(a, w, N, **kw)), C.byref(out)))
+    return dict(zip(("cluster", "clusters"), out))
+
+
+def set_gemm_cluster(mode):
+    """How later GEMM plans pick their cluster size (lseg_debug_set_gemm_cluster): 1 never pair CTAs, 2 the planner's
+    rule (default), 3 pair CTAs wherever possible."""
+    check(load().lseg_debug_set_gemm_cluster(int(mode)))
+
+
 def _attn_out(out, rows, heads, device, what):
     """A caller-given output must be fp16 [rows, heads*64]: the kernel writes exactly that much, unchecked."""
     if out is None:

@@ -3,8 +3,10 @@
 
 Each shape runs on seeded random operands (the timing does not depend on the values), warmed up, then timed with CUDA
 events over enough back-to-back launches to fill at least --min-ms; the median of --reps such windows is reported as
-ms per launch and TFLOP/s (2 M N K taps over that time). The card name and its power limit are printed first: the
-numbers are only meaningful with them.
+ms per launch and TFLOP/s (2 M N K taps over that time). Every shape is timed twice in the same process, with 2-CTA
+clusters wherever possible and with every GEMM unclustered (lseg_debug_set_gemm_cluster modes 3 and 1), the two windows
+alternating; "cl" is the cluster size the planner picks for the shape by default. The card name and its power limit are
+printed first: the numbers are only meaningful with them.
 
 LSEG_GEMM_PROBE (read once per process, see GemmParams::probe) turns parts of the kernel off; run the script once
 without it and once with LSEG_GEMM_PROBE=1 (epilogue skipped) to see how much of each shape's time the epilogue adds.
@@ -43,7 +45,7 @@ def card():
 
 
 def shapes(g):
-    """(name, flops, launch) per shape; every launch writes only buffers allocated here."""
+    """(name, flops, gemm args, gemm keywords) per shape; every launch writes only buffers allocated here."""
     dev = "cuda"
     h = lambda *s: (torch.randn(*s, generator=g, device=dev) * 0.5).half()  # noqa: E731
     f = lambda *s: torch.randn(*s, generator=g, device=dev)  # noqa: E731
@@ -51,7 +53,7 @@ def shapes(g):
 
     def linear(name, M, K, N, **kw):
         a, w, bias = h(M, K), ops.pad_rows(h(N, K) * 0.05), f(N)
-        out.append((name, 2.0 * M * N * K, lambda: ops.gemm(a, w, N, M=M, bias=bias, **kw)))
+        out.append((name, 2.0 * M * N * K, (a, w, N), dict(M=M, bias=bias, **kw)))
 
     x = f(TOKENS, 1024)
     linear("vit qkv      1024->3072 f16", TOKENS, 1024, 3072, out_f16=torch.empty(TOKENS, 3072, device=dev).half())
@@ -65,61 +67,59 @@ def shapes(g):
         xin = h(B, side, side, cin)
         wrn = ops.pad_rows(h(FEAT, 9 * cin) * 0.02)
         o32, r16 = torch.empty(px, FEAT, device=dev), torch.empty(px, FEAT, device=dev).half()
-        out.append((f"layer_rn {side:3d}^ {cin:4d}->256 f32+relu", 2.0 * px * FEAT * 9 * cin,
-                    lambda xin=xin, wrn=wrn, o32=o32, r16=r16: ops.gemm(xin, wrn, FEAT, conv=(3, 1), out_f32=o32,
-                                                                       out_f16_relu=r16, ldc=FEAT)))
+        out.append((f"layer_rn {side:3d}^ {cin:4d}->256 f32+relu", 2.0 * px * FEAT * 9 * cin, (xin, wrn, FEAT),
+                    dict(conv=(3, 1), out_f32=o32, out_f16_relu=r16, ldc=FEAT)))
         t = h(B, side, side, FEAT)
         w3 = ops.pad_rows(h(FEAT, 9 * FEAT) * 0.02)
         sc, sh = f(FEAT).abs() + 0.5, f(FEAT)
         res, t16 = f(px, FEAT), torch.empty(px, FEAT, device=dev).half()
         s32, s16 = torch.empty(px, FEAT, device=dev), torch.empty(px, FEAT, device=dev).half()
         fl = 2.0 * px * FEAT * 9 * FEAT
-        out.append((f"rcu conv1 {side:3d}^ bn relu f16", fl,
-                    lambda t=t, w3=w3, sc=sc, sh=sh, t16=t16: ops.gemm(t, w3, FEAT, conv=(3, 1), scale=sc, bias=sh,
-                                                                      act=ops.ACT_RELU, out_f16=t16, ldc=FEAT)))
-        out.append((f"rcu conv2 {side:3d}^ bn +res f32+relu", fl,
-                    lambda t=t, w3=w3, sc=sc, sh=sh, res=res, s32=s32, s16=s16: ops.gemm(
-                        t, w3, FEAT, conv=(3, 1), scale=sc, bias=sh, res_f32=res, out_f32=s32, out_f16_relu=s16,
-                        ldc=FEAT)))
+        out.append((f"rcu conv1 {side:3d}^ bn relu f16", fl, (t, w3, FEAT),
+                    dict(conv=(3, 1), scale=sc, bias=sh, act=ops.ACT_RELU, out_f16=t16, ldc=FEAT)))
+        out.append((f"rcu conv2 {side:3d}^ bn +res f32+relu", fl, (t, w3, FEAT),
+                    dict(conv=(3, 1), scale=sc, bias=sh, res_f32=res, out_f32=s32, out_f16_relu=s16, ldc=FEAT)))
         a1, w1, b1 = h(px, FEAT), ops.pad_rows(h(FEAT, FEAT) * 0.05), f(FEAT)
-        out.append((f"out_conv  {side:3d}^ 1x1 f32", 2.0 * px * FEAT * FEAT,
-                    lambda a1=a1, w1=w1, b1=b1, o32=o32: ops.gemm(a1, w1, FEAT, bias=b1, out_f32=o32)))
+        out.append((f"out_conv  {side:3d}^ 1x1 f32", 2.0 * px * FEAT * FEAT, (a1, w1, FEAT), dict(bias=b1, out_f32=o32)))
 
     path, wh, bh = h(PIX, FEAT), ops.pad_rows(h(OUT_C, FEAT) * 0.05), f(OUT_C)
     feat16 = torch.empty(PIX, OUT_C, device=dev).half()
     sumsq = torch.empty(PIX, OUT_C // 32, device=dev)
-    out.append(("head1     256->512 f16+sumsq", 2.0 * PIX * OUT_C * FEAT,
-                lambda: ops.gemm(path, wh, OUT_C, bias=bh, out_f16=feat16, out_row_sumsq=sumsq)))
+    out.append(("head1     256->512 f16+sumsq", 2.0 * PIX * OUT_C * FEAT, (path, wh, OUT_C),
+                dict(bias=bh, out_f16=feat16, out_row_sumsq=sumsq)))
     text = ops.pad_rows(h(LABELS, OUT_C) * 0.05)
     logits = torch.empty(B, LABELS, PIX // B, device=dev).half()
     ss = f(PIX, OUT_C // 32).abs() + 1.0
-    out.append(("pixel x text 512->150 nchw", 2.0 * PIX * LABELS * OUT_C,
-                lambda: ops.gemm(feat16, text, LABELS, out_f16=logits, store=ops.STORE_NCHW_T,
-                                 nchw=(PIX // B, LABELS), row_sumsq=ss, row_scale=14.0)))
+    out.append(("pixel x text 512->150 nchw", 2.0 * PIX * LABELS * OUT_C, (feat16, text, LABELS),
+                dict(out_f16=logits, store=ops.STORE_NCHW_T, nchw=(PIX // B, LABELS), row_sumsq=ss, row_scale=14.0)))
     return out
 
 
-def time_launch(fn, min_ms, reps):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
+def window(fn, n):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
-    for _ in range(5):
+    for _ in range(n):
         fn()
     ev1.record()
     ev1.synchronize()
-    n = max(5, int(min_ms / max(ev0.elapsed_time(ev1) / 5, 1e-3)) + 1)
-    times = []
-    for _ in range(reps):
-        ev0.record()
-        for _ in range(n):
+    return ev0.elapsed_time(ev1) / n
+
+
+def time_launch(fn, min_ms, reps):
+    """Median ms per launch with pairs wherever possible (mode 3) and unclustered (mode 1), the windows alternating."""
+    times = {3: [], 1: []}
+    for mode in times:
+        ops.set_gemm_cluster(mode)
+        for _ in range(3):
             fn()
-        ev1.record()
-        ev1.synchronize()
-        times.append(ev0.elapsed_time(ev1) / n)
-    times.sort()
-    return times[len(times) // 2], n
+    torch.cuda.synchronize()
+    n = max(5, int(min_ms / max(window(fn, 5), 1e-3)) + 1)
+    for _ in range(reps):
+        for mode, t in times.items():
+            ops.set_gemm_cluster(mode)
+            t.append(window(fn, n))
+    ops.set_gemm_cluster(2)
+    return {mode: sorted(t)[len(t) // 2] for mode, t in times.items()}, n
 
 
 def main():
@@ -135,11 +135,15 @@ def main():
     print(f"# {name}, power limit / max SM clock: {power}; LSEG_GEMM_PROBE={probe}")
     g = torch.Generator(device="cuda").manual_seed(0)
     rows = []
-    for label, flops, fn in shapes(g):
-        ms, n = time_launch(fn, args.min_ms, args.reps)
-        tf = flops / (ms * 1e-3) / 1e12
-        rows.append({"shape": label, "ms": ms, "tflops": tf, "launches": n})
-        print(f"{label:40s} {ms:9.4f} ms {tf:8.1f} TFLOP/s  ({n} launches per window)")
+    print(f"{'shape':40s} cl {'paired ms':>9s} {'TFLOP/s':>8s} | unclustered {'ms':>9s} {'TFLOP/s':>8s}")
+    for label, flops, gargs, kw in shapes(g):
+        cl = ops.gemm_cluster(*gargs, **kw)["cluster"]
+        ms, n = time_launch(lambda: ops.gemm(*gargs, **kw), args.min_ms, args.reps)
+        tf = {mode: flops / (t * 1e-3) / 1e12 for mode, t in ms.items()}
+        rows.append({"shape": label, "cluster": cl, "ms_paired": ms[3], "tflops_paired": tf[3], "ms_unclustered": ms[1],
+                     "tflops_unclustered": tf[1], "launches": n})
+        print(f"{label:40s} {cl:2d} {ms[3]:9.4f} {tf[3]:8.1f} | {'':11s} {ms[1]:9.4f} {tf[1]:8.1f}  "
+              f"({n} launches per window, {ms[1] / ms[3] - 1:+.1%})")
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"card": name, "power": power, "probe": probe, "shapes": rows}, fh, indent=1)

@@ -408,6 +408,48 @@ int lseg_forward_profiled(lseg_engine* e, const float* x, int B, int H, int W, c
                           long long text_image_stride, float* out, void* stream, float* step_ms, int* step_kind,
                           double* step_flops, int cap, int* count);
 
+/* Encode once, query many times. LSeg.forward splits at the pixel embedding (lseg_net.py:185-191): the image path
+ * (ViT or ResNet trunk, reassemble, decoder, head1) depends on the image only; the pixel x text product, the arch_option
+ * head blocks and the x2 output stage depend on the labels. lseg_encode_image runs the first part into a caller's
+ * buffers; lseg_query runs the second part on them, as often as wanted, with any label set.
+ *
+ * Embedding layout: the engine's own internal pair, for B images of H x W (h = H/2, w = W/2, P = h*w pixels per image,
+ * C = out_c of the weights):
+ *   emb        fp16 [B, h, w, C]     head1's output rows, NOT normalised
+ *   emb_sumsq  fp32 [B, h, w, C/32]  partial squared norms of the fp32 accumulators behind those rows (column chunks of
+ *                                    32), summed in index order where the norm is needed
+ * This pair is what the pixel x text GEMM's epilogue consumes (it applies logit_scale / ||row|| per pixel row), so a
+ * query is bit-identical to the forward of the image that produced it; exporting any other form (normalised, fp32,
+ * NCHW) would round differently and break that identity. lseg_embedding_features converts the pair into the reference's
+ * image_features. Both buffers are 16-byte aligned; an embedding stays valid as long as the caller keeps it (the engine
+ * holds no reference to it) and only for the weights it was encoded with.
+ *
+ * lseg_encode_image: x fp32 NCHW [B,3,H,W] (H, W multiples of 32) -> emb, emb_sumsq. Same launches as lseg_forward's
+ * image path; head1 stores straight into the caller's buffers. */
+int lseg_encode_image(lseg_engine* e, const float* x, int B, int H, int W,
+                      void* emb /* fp16 [B,H/2,W/2,out_c] */, float* emb_sumsq /* fp32 [B,H/2,W/2,out_c/32] */, void* stream);
+
+/* The label-dependent tail of LSeg.forward on an embedding of B images of H x W. text / K / text_image_stride as in
+ * lseg_forward. Outputs, each nullable, at least one requested; each equals what the corresponding forward entry point
+ * writes for the image that produced `emb`, bit for bit:
+ *   logits  fp32 [B,K,H,W]  (lseg_forward)
+ *   mask    int64 [B,H,W]   (lseg_forward_argmax)
+ *   stats   int64 [G, 3*nclass + 2], accumulated, with target int64 [B,H,W] and group int32 [B] or NULL
+ *           (lseg_forward_segstats; W <= 1024). target, group and stats are all NULL, or target and stats are given.
+ * Every argument is checked, and rejected by name, before the first launch. A query at a shape the engine never ran a
+ * forward at allocates only the tail's buffers (fp16 [B,K,H/2,W/2] low-res logits; fp32 head-block planes with
+ * arch_option 1 / 2), never the image path's activations. */
+int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W,
+               const void* text, int K, long long text_image_stride,
+               float* logits, long long* mask,
+               const long long* target, const int* group, int nclass, int G, long long* stats,
+               void* stream);
+
+/* The reference's normalised pixel embedding image_features (lseg_net.py:187-191) from an embedding pair of B images
+ * with an h x w grid: out fp32 NCHW [B, C, h, w] = emb * rsqrt(sum of the C/32 partials, in index order). C in
+ * {512, 768}; h*w a multiple of 4; emb and out 16-byte aligned. No engine needed. */
+int lseg_embedding_features(const void* emb, const float* emb_sumsq, int B, int h, int w, int C, float* out, void* stream);
+
 /* Introspection for tests: copies of intermediate activations of the last forward (device pointers
  * into the workspace, valid until the next forward). name: "tap0".."tap3" fp32 [B,N,1024];
  * "path1" fp16 NHWC [B,H/2,W/2,256]; "logits_lr" fp16 [B,K,H/2,W/2]. Returns NULL if unknown. */

@@ -97,6 +97,7 @@ SYMBOLS = [
     "lseg_p2p_wait",
     "lseg_eval_make_crops", "lseg_eval_canvas", "lseg_eval_resize_add", "lseg_preprocess",
     "lseg_seg_stats_scores", "lseg_seg_stats_mask", "lseg_forward_segstats",
+    "lseg_encode_image", "lseg_query", "lseg_embedding_features",
 ]
 
 _lib = None
@@ -196,6 +197,13 @@ def load(build_if_missing=True):
     lib.lseg_forward_segstats.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                           C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
+    lib.lseg_encode_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]
+    lib.lseg_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                               C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                               C.c_void_p, C.c_void_p]
+    lib.lseg_embedding_features.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_void_p]
     lib.lseg_last_launch_count.argtypes = [C.c_void_p]
     lib.lseg_forward_profiled.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                           C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_float),

@@ -83,30 +83,45 @@ struct ImagePlan {
   int B = 0, H = 0, W = 0;
   int epoch = 0;  // g_plan_epoch at build time (options baked into the GEMM plans)
   Arena arena;
-  std::vector<Step> steps;
+  std::vector<Step> steps;  // the trunk up to (not including) head1
   std::map<std::string, const void*> debug;
-  // head buffers needed by the per-call tail
+  // head1 (lseg_net.py:185): path1 -> the pixel embedding. forward writes the plan's own featn / feat_sumsq;
+  // lseg_encode_image writes a caller's buffers, with one GEMM plan (host-encoded tensor maps) per destination
+  GemmDesc head1_desc;
+  float* head1_ws = nullptr;  // split-K workspace of head1 (shared by its plans: calls on an engine are stream-ordered)
+  std::map<std::pair<const void*, const void*>, GemmPlan> head1;
   __half* featn = nullptr;
   float* feat_sumsq = nullptr;
-  __half* logits_lr = nullptr;  // own cudaMalloc (grows with K), not part of the arena
+  unsigned long long last_use = 0;
+  ~ImagePlan() { arena.release(); }
+};
+
+// Buffers of the label-dependent tail at one (B, H, W): independent of the trunk's activation arena, so a query on a
+// stored embedding at a shape the engine never ran a forward at allocates only these.
+struct TailWs {
+  int B = 0, H = 0, W = 0;
+  int epoch = 0;  // g_plan_epoch of the cached pixel x text plans
+  __half* logits_lr = nullptr;  // fp16 [B,K,H/2,W/2], grows with K
   size_t logits_cap_k = 0;
-  float* head_ws[2] = {nullptr, nullptr};  // arch_option 1/2: fp32 [B,K,h,w] ping-pong (own cudaMalloc, grows with K)
+  float* head_ws[2] = {nullptr, nullptr};  // arch_option 1/2: fp32 [B,K,h,w] ping-pong, grows with K
   float* head_cmax = nullptr;              // [B,h,w]
   size_t head_cap_k = 0;
-  // pixel x text GEMM plans (host-encoded tensor maps) keyed by (text pointer, K, per-image stride, output pointer)
+  // pixel x text GEMM plans (host-encoded tensor maps) keyed by (text pointer, K, per-image stride, output pointer,
+  // embedding pointers)
   struct CorrKey {
     const void* text;
     int K;
     long long stride;
     const void* out;
+    const void* emb;
+    const void* sumsq;
     bool operator<(const CorrKey& o) const {
-      return std::tie(text, K, stride, out) < std::tie(o.text, o.K, o.stride, o.out);
+      return std::tie(text, K, stride, out, emb, sumsq) < std::tie(o.text, o.K, o.stride, o.out, o.emb, o.sumsq);
     }
   };
   std::map<CorrKey, std::vector<std::pair<GemmPlan, double>>> corr;
   unsigned long long last_use = 0;
-  ~ImagePlan() {
-    arena.release();
+  ~TailWs() {
     if (logits_lr) cudaFree(logits_lr);
     for (float* p : head_ws)
       if (p) cudaFree(p);
@@ -131,6 +146,8 @@ struct lseg_engine {
   static constexpr int kMaxImagePlans = 3;
   std::vector<std::unique_ptr<lseg::ImagePlan>> plans;
   lseg::ImagePlan* img = nullptr;  // the plan of the last forward (debug buffers)
+  static constexpr int kMaxTails = 3;
+  std::vector<std::unique_ptr<lseg::TailWs>> tails;  // least-recently-used, like the image plans
   unsigned long long use_counter = 0;
   std::unique_ptr<lseg::TextPlan> txt;
   std::map<std::pair<int, int>, float*> pos_cache;
@@ -708,12 +725,29 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t 
   LSEG_ALLOC(featn, __half, BP * OC);
   LSEG_ALLOC(feat_sumsq, float, BP * (OC / 32));  // [row, out_c/32] partial squared norms
   {
-    GemmEpi e = epi_none();
-    e.bias = w.head1.b;
-    e.out_f16 = featn;
-    e.out_row_sumsq = feat_sumsq;
-    e.ldc = OC;
-    if (add_gemm(steps, path1_f16, 256, (int)BP, (int)BP, w.head1, e)) return -1;
+    GemmDesc& d = plan->head1_desc;
+    memset(&d, 0, sizeof(d));
+    d.a = path1_f16;
+    d.lda = 256;
+    d.a_rows = (int)BP;
+    d.w = static_cast<const __half*>(w.head1.w);
+    d.w_rows = w.head1.rows;
+    d.M = (int)BP;
+    d.N = w.head1.out;
+    d.K = w.head1.in;
+    d.e = epi_none();
+    d.e.bias = w.head1.b;
+    d.e.out_f16 = featn;
+    d.e.out_row_sumsq = feat_sumsq;
+    d.e.ldc = OC;
+    GemmPlan gp;
+    if (gemm_plan(d, &gp)) return -1;
+    if (gp.ws_bytes) {
+      LSEG_ALLOC(ws, float, gp.ws_bytes / sizeof(float));
+      plan->head1_ws = ws;
+      gemm_set_workspace(&gp, ws);
+    }
+    plan->head1.emplace(std::make_pair(static_cast<const void*>(featn), static_cast<const void*>(feat_sumsq)), gp);
   }
   plan->featn = featn;
   plan->feat_sumsq = feat_sumsq;
@@ -744,65 +778,157 @@ struct Profile {
   }
 };
 
-static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, cudaStream_t stream,
-                       Profile* prof = nullptr) {
-  if (ensure_init()) return -1;
-  if (H % 32 != 0 || W % 32 != 0 || H <= 0 || W <= 0) {
-    // the reference fails deep inside skip_add.add (lseg_blocks.py:347) for odd token grids
-    set_error("lseg_forward: H=%d, W=%d must be positive multiples of 32", H, W);
-    return -1;
+// A launch of the forward or query path: counted, and timed when profiling.
+static int note_launch(Profile* prof, int* launches, int kind, double flops, cudaStream_t stream) {
+  ++*launches;
+  if (prof) {
+    if (prof->mark(stream)) return -1;
+    prof->kind.push_back(kind);
+    prof->flops.push_back(flops);
   }
-  if (ctx.K <= 0) {
-    set_error("lseg_forward: K=%d labels", ctx.K);
-    return -1;
-  }
-  LSEG_CHECK_CUDA(cudaSetDevice(eng->device));
-  if (ensure_init()) return -1;
+  return 0;
+}
+
+static int check_image_shape(const char* fn, int B, int H, int W) {
+  if (B <= 0) return set_error("%s: B=%d must be positive", fn, B), -1;
+  if (H % 32 != 0 || W % 32 != 0 || H <= 0 || W <= 0)  // the reference fails deep inside skip_add.add
+    return set_error("%s: H=%d, W=%d must be positive multiples of 32", fn, H, W), -1;  // (lseg_blocks.py:347)
+  return 0;
+}
+
+// The image plan for (B, H, W), built on first use; plans built under other baked-in options are dropped.
+static ImagePlan* image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t stream) {
   eng->img = nullptr;
   for (size_t i = 0; i < eng->plans.size();) {
     ImagePlan* pl = eng->plans[i].get();
     if (pl->epoch != g_plan_epoch) {  // an option baked into the GEMM plans changed
-      LSEG_CHECK_CUDA(cudaStreamSynchronize(stream));
+      if (cudaStreamSynchronize(stream) != cudaSuccess) return set_error("image plan: stream sync failed"), nullptr;
       eng->plans.erase(eng->plans.begin() + i);
       continue;
     }
     if (pl->B == B && pl->H == H && pl->W == W) eng->img = pl;
     ++i;
   }
-  if (!eng->img && build_image_plan(eng, B, H, W, stream)) return -1;
-  ImagePlan& plan = *eng->img;
-  plan.last_use = ++eng->use_counter;
-  const int h2 = H / 2, w2 = W / 2;
-  const long long P = static_cast<long long>(h2) * w2;
-  if (!ctx.out_lr && (!plan.logits_lr || plan.logits_cap_k < (size_t)ctx.K)) {
-    if (plan.logits_lr) {
-      LSEG_CHECK_CUDA(cudaStreamSynchronize(stream));
-      LSEG_CHECK_CUDA(cudaFree(plan.logits_lr));
-      plan.logits_lr = nullptr;
-      plan.corr.clear();
+  if (!eng->img && build_image_plan(eng, B, H, W, stream)) return nullptr;
+  eng->img->last_use = ++eng->use_counter;
+  return eng->img;
+}
+
+// The trunk: plan.steps, then head1 into (emb, sumsq) — fp16 [B*P, out_c] un-normalised rows and their fp32 partial
+// squared norms [B*P, out_c/32] — the plan's own featn / feat_sumsq for a forward, a caller's buffers for
+// lseg_encode_image. Same launches and bits either way; only head1's output address differs.
+static int run_trunk(lseg_engine* eng, ImagePlan& plan, const CallCtx& ctx, __half* emb, float* sumsq, cudaStream_t stream,
+                     Profile* prof, int* launches) {
+  auto key = std::make_pair(static_cast<const void*>(emb), static_cast<const void*>(sumsq));
+  auto it = plan.head1.find(key);
+  if (it == plan.head1.end()) {
+    if (plan.head1.size() > 16) {  // keep the plan of the own buffers
+      auto own = plan.head1.find(std::make_pair(static_cast<const void*>(plan.featn), static_cast<const void*>(plan.feat_sumsq)));
+      GemmPlan keep = own->second;
+      plan.head1.clear();
+      plan.head1.emplace(own->first, keep);
     }
-    void* p = nullptr;
-    if (cudaMalloc(&p, sizeof(__half) * (size_t)B * ctx.K * P) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("logits workspace allocation failed");
-      return -1;
-    }
-    plan.logits_lr = static_cast<__half*>(p);
-    plan.logits_cap_k = ctx.K;
+    GemmDesc d = plan.head1_desc;
+    d.e.out_f16 = emb;
+    d.e.out_row_sumsq = sumsq;
+    GemmPlan gp;
+    if (gemm_plan(d, &gp)) return -1;
+    if (gp.ws_bytes) gemm_set_workspace(&gp, plan.head1_ws);
+    it = plan.head1.emplace(key, gp).first;
   }
-  __half* lr = ctx.out_lr ? ctx.out_lr : plan.logits_lr;
-  plan.debug["logits_lr"] = lr;
-  int launches = 0;
   if (prof && prof->mark(stream)) return -1;
   for (auto& st : plan.steps) {
     if (st(ctx, stream)) return -1;
-    if (st.kind != KIND_MEMSET) ++launches;  // count our kernels only
+    if (st.kind != KIND_MEMSET) ++*launches;  // count our kernels only
     if (prof) {
       if (prof->mark(stream)) return -1;
       prof->kind.push_back(st.kind);
       prof->flops.push_back(st.flops);
     }
   }
+  const GemmDesc& d = plan.head1_desc;
+  if (gemm_run(it->second, stream)) return -1;
+  return note_launch(prof, launches, KIND_GEMM, 2.0 * d.M * d.N * static_cast<double>(d.K), stream);
+}
+
+// The tail workspace for (B, H, W) with room for K labels.
+static TailWs* tail_ws(lseg_engine* eng, int B, int H, int W, int K, bool need_lr, cudaStream_t stream) {
+  TailWs* t = nullptr;
+  for (auto& p : eng->tails)
+    if (p->B == B && p->H == H && p->W == W) t = p.get();
+  if (!t) {
+    if (static_cast<int>(eng->tails.size()) >= lseg_engine::kMaxTails) {
+      size_t victim = 0;
+      for (size_t i = 1; i < eng->tails.size(); ++i)
+        if (eng->tails[i]->last_use < eng->tails[victim]->last_use) victim = i;
+      // the victim's buffers may still be in use by queued work
+      if (cudaStreamSynchronize(stream) != cudaSuccess) return set_error("tail workspace: stream sync failed"), nullptr;
+      eng->tails.erase(eng->tails.begin() + victim);
+    }
+    eng->tails.emplace_back(new TailWs());
+    t = eng->tails.back().get();
+    t->B = B;
+    t->H = H;
+    t->W = W;
+    t->epoch = g_plan_epoch;
+  }
+  if (t->epoch != g_plan_epoch) {  // an option baked into the GEMM plans changed
+    t->corr.clear();
+    t->epoch = g_plan_epoch;
+  }
+  t->last_use = ++eng->use_counter;
+  const size_t P = static_cast<size_t>(H / 2) * (W / 2);
+  if (need_lr && (!t->logits_lr || t->logits_cap_k < (size_t)K)) {
+    if (t->logits_lr) {
+      if (cudaStreamSynchronize(stream) != cudaSuccess) return set_error("tail workspace: stream sync failed"), nullptr;
+      cudaFree(t->logits_lr);
+      t->logits_lr = nullptr;
+      t->corr.clear();
+    }
+    void* p = nullptr;
+    if (cudaMalloc(&p, sizeof(__half) * (size_t)B * K * P) != cudaSuccess) {
+      cudaGetLastError();
+      return set_error("logits workspace allocation failed"), nullptr;
+    }
+    t->logits_lr = static_cast<__half*>(p);
+    t->logits_cap_k = K;
+  }
+  const int arch = eng->w.arch_option;
+  if ((arch == 1 || arch == 2) && (!t->head_ws[0] || t->head_cap_k < (size_t)K)) {
+    if (cudaStreamSynchronize(stream) != cudaSuccess) return set_error("tail workspace: stream sync failed"), nullptr;
+    for (int i = 0; i < 2; ++i) {
+      if (t->head_ws[i]) cudaFree(t->head_ws[i]);
+      t->head_ws[i] = nullptr;
+      if (cudaMalloc(&t->head_ws[i], sizeof(float) * (size_t)B * K * P) != cudaSuccess) {
+        cudaGetLastError();
+        return set_error("head block workspace allocation failed"), nullptr;
+      }
+    }
+    if (!t->head_cmax && cudaMalloc(&t->head_cmax, sizeof(float) * (size_t)B * P) != cudaSuccess) {
+      cudaGetLastError();
+      return set_error("head block workspace allocation failed"), nullptr;
+    }
+    t->head_cap_k = K;
+  }
+  return t;
+}
+
+// The label-dependent tail of LSeg.forward on a pixel embedding (emb, sumsq) of B images of H x W: the pixel x text
+// GEMM, the arch_option head blocks and the x2 output stage (logits / argmax / metric counters). The one implementation
+// behind every forward entry point and lseg_query. *lr_out: where the fp16 low-res logits went.
+static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, const __half* emb, const float* sumsq,
+                    cudaStream_t stream, Profile* prof, int* launches, __half** lr_out) {
+  const int arch = eng->w.arch_option;
+  if (ctx.out_lr && (arch == 1 || arch == 2)) {
+    set_error("lseg_forward_lowres: the fp16 low-res logits are not the network output when arch_option is %d", arch);
+    return -1;
+  }
+  TailWs* t = tail_ws(eng, B, H, W, ctx.K, !ctx.out_lr, stream);
+  if (!t) return -1;
+  const int h2 = H / 2, w2 = W / 2;
+  const long long P = static_cast<long long>(h2) * w2;
+  __half* lr = ctx.out_lr ? ctx.out_lr : t->logits_lr;
+  *lr_out = lr;
   // ---- pixel x text correlation (lseg_net.py:194-196): fp16 GEMM, fp16 result, NCHW store ----
   // One label set for all images (text_image_stride == 0): one GEMM over all B*P pixel rows.
   // One label block per image (zero-shot path, lseg_net_zs.py:196-210; rows [b*stride, b*stride + K) of `text`):
@@ -811,10 +937,10 @@ static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W
   // so this costs the same tile as one image's block and replaces B launches by one. Falls back to one launch per
   // image when B*stride exceeds one 256-column tile.
   {
-    ImagePlan::CorrKey key{ctx.text, ctx.K, ctx.text_image_stride, lr};
-    auto it = plan.corr.find(key);
-    if (it == plan.corr.end()) {
-      if (plan.corr.size() > 16) plan.corr.clear();
+    TailWs::CorrKey key{ctx.text, ctx.K, ctx.text_image_stride, lr, emb, sumsq};
+    auto it = t->corr.find(key);
+    if (it == t->corr.end()) {
+      if (t->corr.size() > 16) t->corr.clear();
       std::vector<std::pair<GemmPlan, double>> plans;
       const long long stride = ctx.text_image_stride;
       const bool grouped = stride > 0 && static_cast<long long>(B) * stride <= 256;
@@ -825,7 +951,7 @@ static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W
         const long long rows = (groups == 1) ? static_cast<long long>(B) * P : P;
         const int n_cols = grouped ? static_cast<int>(B * stride) : ctx.K;
         const int OC = eng->w.out_c;
-        d.a = plan.featn + static_cast<long long>(g) * P * OC;
+        d.a = emb + static_cast<long long>(g) * P * OC;
         d.lda = OC;
         d.a_rows = (int)rows;
         d.w = ctx.text + static_cast<long long>(g) * stride * OC;
@@ -839,60 +965,36 @@ static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W
         d.e.nchw_p = (int)P;
         d.e.nchw_k = ctx.K;
         d.e.nchw_group = grouped ? (int)stride : 0;
-        d.e.row_sumsq = plan.feat_sumsq + static_cast<long long>(g) * P * (OC / 32);
+        d.e.row_sumsq = sumsq + static_cast<long long>(g) * P * (OC / 32);
         d.e.row_sumsq_parts = OC / 32;
         d.e.row_scale = eng->w.logit_scale;
         GemmPlan gp;
         if (gemm_plan(d, &gp)) return -1;
         plans.emplace_back(gp, 2.0 * rows * n_cols * static_cast<double>(OC));
       }
-      it = plan.corr.emplace(key, std::move(plans)).first;
+      it = t->corr.emplace(key, std::move(plans)).first;
     }
     for (auto& pr : it->second) {
       if (gemm_run(pr.first, stream)) return -1;
-      ++launches;
-      if (prof) {
-        if (prof->mark(stream)) return -1;
-        prof->kind.push_back(KIND_GEMM);
-        prof->flops.push_back(pr.second);
-      }
+      if (note_launch(prof, launches, KIND_GEMM, pr.second, stream)) return -1;
     }
   }
   // ---- optional head blocks on the fp32 view of the low-res logits (arch_option 1 / 2, lseg_net.py:198-201) ----
   const float* lr32 = nullptr;
-  const int arch = eng->w.arch_option;
   if (arch == 1 || arch == 2) {
-    if (ctx.out_lr) {
-      set_error("lseg_forward_lowres: the fp16 low-res logits are not the network output when arch_option is %d", arch);
-      return -1;
-    }
-    if (!plan.head_ws[0] || plan.head_cap_k < (size_t)ctx.K) {
-      LSEG_CHECK_CUDA(cudaStreamSynchronize(stream));
-      for (int i = 0; i < 2; ++i) {
-        if (plan.head_ws[i]) cudaFree(plan.head_ws[i]);
-        plan.head_ws[i] = nullptr;
-        LSEG_CHECK_CUDA(cudaMalloc(&plan.head_ws[i], sizeof(float) * (size_t)B * ctx.K * P));
-      }
-      if (!plan.head_cmax) LSEG_CHECK_CUDA(cudaMalloc(&plan.head_cmax, sizeof(float) * (size_t)B * P));
-      plan.head_cap_k = ctx.K;
-    }
     HeadBlockW hw;
     for (int i = 0; i < 9; ++i) hw.w[i] = eng->w.head_block_w[i];
     hw.bias = eng->w.head_block_b;
     const int depth = eng->w.block_depth > 1 ? eng->w.block_depth : 1;  // range(block_depth - 1) + the final call
     for (int dpt = 0; dpt < depth; ++dpt) {
       const int act = (dpt + 1 < depth) ? eng->w.head_act : HEAD_ACT_NONE;
-      float* dst = plan.head_ws[dpt & 1];
-      int rc = (dpt == 0) ? launch_head_block(lr, plan.head_cmax, dst, B, ctx.K, h2, w2, hw, arch, act, stream)
-                          : launch_head_block(static_cast<const float*>(plan.head_ws[(dpt - 1) & 1]), plan.head_cmax, dst,
+      float* dst = t->head_ws[dpt & 1];
+      int rc = (dpt == 0) ? launch_head_block(lr, t->head_cmax, dst, B, ctx.K, h2, w2, hw, arch, act, stream)
+                          : launch_head_block(static_cast<const float*>(t->head_ws[(dpt - 1) & 1]), t->head_cmax, dst,
                                               B, ctx.K, h2, w2, hw, arch, act, stream);
       if (rc) return -1;
-      launches += (arch == 1) ? 2 : 1;
-      if (prof) {
-        if (prof->mark(stream)) return -1;
-        prof->kind.push_back(KIND_EW);
-        prof->flops.push_back(0.0);
-      }
+      if (arch == 1) ++*launches;  // bottleneck_block: channel max + conv
+      if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
       lr32 = dst;
     }
   }
@@ -902,35 +1004,40 @@ static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W
     if (lr32 ? launch_upsample2x_nchw(lr32, ctx.out, planes, h2, w2, stream)
              : launch_upsample2x_nchw(lr, ctx.out, planes, h2, w2, stream))
       return -1;
-    ++launches;
-    if (prof) {
-      if (prof->mark(stream)) return -1;
-      prof->kind.push_back(KIND_EW);
-      prof->flops.push_back(0.0);
-    }
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
   }
   // ---- fused output_conv + torch.max(.., 1)[1] (SURVEY.md 8(f) row 2): the fp32 logits are never materialised ----
   if (ctx.seg) {  // ... and counted into the metric rows in the same kernel
     if (lr32 ? launch_upsample2x_segstats(lr32, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream)
              : launch_upsample2x_segstats(lr, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream))
       return -1;
-    ++launches;
-    if (prof) {
-      if (prof->mark(stream)) return -1;
-      prof->kind.push_back(KIND_EW);
-      prof->flops.push_back(0.0);
-    }
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
   } else if (ctx.out_mask) {
     if (lr32 ? launch_upsample2x_argmax(lr32, ctx.out_mask, B, ctx.K, h2, w2, stream)
              : launch_upsample2x_argmax(lr, ctx.out_mask, B, ctx.K, h2, w2, stream))
       return -1;
-    ++launches;
-    if (prof) {
-      if (prof->mark(stream)) return -1;
-      prof->kind.push_back(KIND_EW);
-      prof->flops.push_back(0.0);
-    }
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
   }
+  return 0;
+}
+
+static int run_forward(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, cudaStream_t stream,
+                       Profile* prof = nullptr) {
+  if (ensure_init()) return -1;
+  if (check_image_shape("lseg_forward", B, H, W)) return -1;
+  if (ctx.K <= 0) {
+    set_error("lseg_forward: K=%d labels", ctx.K);
+    return -1;
+  }
+  LSEG_CHECK_CUDA(cudaSetDevice(eng->device));
+  if (ensure_init()) return -1;
+  ImagePlan* plan = image_plan(eng, B, H, W, stream);
+  if (!plan) return -1;
+  int launches = 0;
+  if (run_trunk(eng, *plan, ctx, plan->featn, plan->feat_sumsq, stream, prof, &launches)) return -1;
+  __half* lr = nullptr;
+  if (run_tail(eng, ctx, B, H, W, plan->featn, plan->feat_sumsq, stream, prof, &launches, &lr)) return -1;
+  plan->debug["logits_lr"] = lr;
   eng->last_launches = launches;
   return 0;
 }
@@ -1240,6 +1347,94 @@ int lseg_forward_profiled(lseg_engine* e, const float* x, int B, int H, int W, c
   for (cudaEvent_t ev : prof.ev) cudaEventDestroy(ev);
   *count = n;
   return rc;
+}
+
+int lseg_encode_image(lseg_engine* e, const float* x, int B, int H, int W, void* emb, float* emb_sumsq, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_encode_image";
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!x) return set_error("%s: null x", fn), -1;
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 16) return set_error("%s: emb_sumsq must be 16-byte aligned", fn), -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  if (ensure_init()) return -1;
+  LSEG_CHECK_CUDA(cudaSetDevice(e->device));
+  if (ensure_init()) return -1;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  ImagePlan* plan = image_plan(e, B, H, W, s);
+  if (!plan) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.x = x;
+  int launches = 0;
+  if (run_trunk(e, *plan, ctx, static_cast<__half*>(emb), emb_sumsq, s, nullptr, &launches)) return -1;
+  e->last_launches = launches;
+  return 0;
+}
+
+int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W, const void* text, int K,
+               long long text_image_stride, float* logits, long long* mask, const long long* target, const int* group,
+               int nclass, int G, long long* stats, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_query";
+  // every rule is checked here, before the first launch
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (!text) return set_error("%s: null text", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 16) return set_error("%s: emb_sumsq must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(text) % 16) return set_error("%s: text must be 16-byte aligned", fn), -1;
+  if (logits && reinterpret_cast<uintptr_t>(logits) % 16) return set_error("%s: logits must be 16-byte aligned", fn), -1;
+  if (mask && reinterpret_cast<uintptr_t>(mask) % 8) return set_error("%s: mask must be 8-byte aligned", fn), -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  if (K <= 0) return set_error("%s: K=%d labels must be positive", fn, K), -1;
+  if (text_image_stride < 0 || (text_image_stride > 0 && text_image_stride < K))
+    return set_error("%s: text_image_stride=%lld must be 0 or >= K=%d", fn, text_image_stride, K), -1;
+  const bool seg = target || stats || group;
+  if (!logits && !mask && !seg) return set_error("%s: no output requested (logits, mask or stats)", fn), -1;
+  SegStatsArgs st{target, group, stats, nclass, G};
+  if (seg) {
+    if (seg_stats_check(fn, emb, st, B, H, W)) return -1;
+    if (W > 2 * kUpMaxW) return set_error("%s: W=%d must be <= %d with stats", fn, W, 2 * kUpMaxW), -1;
+  }
+  if (ensure_init()) return -1;
+  LSEG_CHECK_CUDA(cudaSetDevice(e->device));
+  if (ensure_init()) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = K;
+  ctx.text_image_stride = text_image_stride;
+  ctx.out = logits;
+  ctx.out_mask = mask;
+  ctx.seg = seg ? &st : nullptr;
+  int launches = 0;
+  __half* lr = nullptr;
+  if (run_tail(e, ctx, B, H, W, static_cast<const __half*>(emb), emb_sumsq, static_cast<cudaStream_t>(stream), nullptr,
+               &launches, &lr))
+    return -1;
+  e->last_launches = launches;
+  return 0;
+}
+
+int lseg_embedding_features(const void* emb, const float* emb_sumsq, int B, int h, int w, int C, float* out,
+                            void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_embedding_features";
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (!out) return set_error("%s: null out", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 4) return set_error("%s: emb_sumsq must be 4-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(out) % 16) return set_error("%s: out must be 16-byte aligned", fn), -1;
+  if (B <= 0 || h <= 0 || w <= 0) return set_error("%s: B=%d, h=%d, w=%d must be positive", fn, B, h, w), -1;
+  if (C != 512 && C != 768) return set_error("%s: C=%d must be 512 or 768", fn, C), -1;
+  if (ensure_init()) return -1;
+  return launch_embed_features(static_cast<const __half*>(emb), emb_sumsq, out, B, static_cast<long long>(h) * w, C,
+                               static_cast<cudaStream_t>(stream));
 }
 
 const void* lseg_debug_buffer(lseg_engine* e, const char* name) {

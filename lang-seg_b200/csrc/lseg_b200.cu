@@ -17,6 +17,7 @@
 #include "text_attn.cuh"
 #include "p2p.cuh"
 #include "evaluator.cuh"
+#include "embed.cuh"
 
 namespace lseg {
 

@@ -11,6 +11,44 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def check_embedding(emb, sumsq, device=None, out_c=None):
+    """Validates an embedding pair (include/lseg_b200.h) -> (B, H, W) of the images it encodes."""
+    if not isinstance(emb, torch.Tensor) or not isinstance(sumsq, torch.Tensor):
+        raise ValueError("emb and sumsq must be tensors")
+    device = emb.device if device is None else device
+    if emb.device != device or sumsq.device != device or device.type != "cuda":
+        raise ValueError(f"embedding is on {emb.device} / {sumsq.device}, expected {device} (CUDA)")
+    c = emb.shape[-1] if out_c is None else out_c
+    if (emb.dtype != torch.float16 or emb.dim() != 4 or emb.shape[3] != c or c not in (512, 768) or
+            not emb.is_contiguous()):
+        raise ValueError(f"emb must be a contiguous float16 [B,H/2,W/2,{c}] tensor (out_c 512 or 768), got {emb.dtype} "
+                         f"{tuple(emb.shape)}")
+    want = tuple(emb.shape[:3]) + (c // 32,)
+    if sumsq.dtype != torch.float32 or tuple(sumsq.shape) != want or not sumsq.is_contiguous():
+        raise ValueError(f"sumsq must be a contiguous float32 {want} tensor, got {sumsq.dtype} {tuple(sumsq.shape)}")
+    b, h2, w2, _ = emb.shape
+    if b == 0 or h2 % 16 or w2 % 16:
+        raise ValueError(f"emb grid {h2}x{w2} of {b} images: not the embedding of H, W multiples of 32")
+    return b, 2 * h2, 2 * w2
+
+
+def embedding_features(emb, sumsq, out=None):
+    """The reference's normalised image_features fp32 [B,C,H/2,W/2] (lseg_net.py:187-191) of an embedding pair: the
+    export kernel of liblseg_b200.so, no engine needed. Enqueues on the current stream."""
+    b, h, w = check_embedding(emb, sumsq)
+    c = emb.shape[3]
+    shape = (b, c, h // 2, w // 2)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=emb.device)
+    elif out.device != emb.device or out.dtype != torch.float32 or tuple(out.shape) != shape or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous float32 {shape} tensor on {emb.device}")
+    lib = _lib.load()
+    with torch.cuda.device(emb.device):
+        _lib.check(lib.lseg_embedding_features(C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()), b, h // 2,
+                                               w // 2, c, C.c_void_p(out.data_ptr()), _stream()))
+    return out
+
+
 class Engine:
     """Owns the packed weights and the native engine for one CUDA device."""
 
@@ -146,6 +184,52 @@ class Engine:
                                                       C.c_void_p(target.data_ptr()), gp, nclass, stats.shape[0],
                                                       C.c_void_p(stats.data_ptr()), mp, lp, _stream()))
         return stats
+
+    def encode_image(self, x):
+        """The image path of forward (trunk, decoder, head1) -> the pixel embedding pair (emb fp16 [B,H/2,W/2,out_c],
+        sumsq fp32 [B,H/2,W/2,out_c/32]); layout in include/lseg_b200.h. Enqueues on the current stream."""
+        self._check_input(x)
+        x = x.contiguous()
+        b, _, h, w = x.shape
+        emb = torch.empty((b, h // 2, w // 2, self.out_c), dtype=torch.float16, device=self.device)
+        sumsq = torch.empty((b, h // 2, w // 2, self.out_c // 32), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_encode_image(self.handle, C.c_void_p(x.data_ptr()), b, h, w,
+                                                  C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()), _stream()))
+        return emb, sumsq
+
+    def query(self, emb, sumsq, text, k, text_image_stride=0, logits=None, mask=None, target=None, stats=None,
+              nclass=0, group=None):
+        """The label-dependent tail of forward on a stored embedding: writes the fp32 logits [B,K,H,W] (as forward), the
+        int64 mask [B,H,W] (as forward_argmax) and / or adds the metric counters of the mask against target to stats (as
+        forward_stats) — whichever tensors are passed, at least one. Enqueues on the current stream."""
+        from .ops import _check_stats, _group_ptr
+        b, h, w = check_embedding(emb, sumsq, self.device, self.out_c)
+        if logits is None and mask is None and stats is None:
+            raise ValueError("query: no output requested (logits, mask or stats)")
+        for name, t, dt, shape in (("mask", mask, torch.int64, (b, h, w)), ("logits", logits, torch.float32, (b, k, h, w))):
+            if t is not None and (t.device != self.device or t.dtype != dt or tuple(t.shape) != shape or
+                                  not t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous {dt} {shape} tensor on {self.device}")
+        tp = gp = sp = None
+        g = 0
+        if stats is not None or target is not None:
+            if stats is None or target is None:
+                raise ValueError("query: target and stats go together")
+            _check_stats(stats, nclass)
+            if target.device != self.device or target.dtype != torch.int64 or tuple(target.shape) != (b, h, w):
+                raise ValueError(f"target must be int64 [B,H,W] = {(b, h, w)} on {self.device}")
+            if stats.device != self.device or not stats.is_contiguous():
+                raise ValueError(f"stats must be a contiguous tensor on {self.device}")
+            target = target.contiguous()
+            g, gp = _group_ptr(group, stats, b)
+            tp, sp = C.c_void_p(target.data_ptr()), C.c_void_p(stats.data_ptr())
+        lp = C.c_void_p(logits.data_ptr()) if logits is not None else None
+        mp = C.c_void_p(mask.data_ptr()) if mask is not None else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_query(self.handle, C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()), b, h, w,
+                                           C.c_void_p(text.data_ptr()), k, text_image_stride, lp, mp, tp, gp,
+                                           nclass, stats.shape[0] if stats is not None else 0, sp, _stream()))
 
     def forward_profiled(self, x, text, k, text_image_stride=0, out=None):
         """One forward with CUDA events around every launch. Returns (out, [(ms, kind, flops), ...])."""

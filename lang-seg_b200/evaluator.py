@@ -94,43 +94,92 @@ class MultiScaleEvaluator:
         return {"height": height, "width": width, "whole": False, "origins": origins}
 
     # ---- fused device path: csrc/evaluator.cuh through the C ABI ----
+    def _windows(self, h, w):
+        """Per-scale geometry, the window list of every network input (plain and flipped, scale by scale) and the first
+        row of each scale in it."""
+        geo = [self._geometry(h, w, scale) for scale in self.scales]
+        rows, first = [], []
+        for g in geo:
+            first.append(len(rows))
+            for (h0, w0) in g["origins"]:
+                rows.append([g["height"], g["width"], h0, w0, 0, len(rows)])
+                if self.flip:
+                    rows.append([g["height"], g["width"], h0, w0, 1, len(rows)])
+        return geo, rows, first
+
+    def _crops(self, image, rows):
+        """Every network input of every scale, built by ONE launch: crops fp32 [len(rows),3,crop,crop]."""
+        import ctypes as C
+        from . import _lib
+        dev = image.device
+        _, _, h, w = image.shape
+        crop = self.crop_size
+        img = image[0].contiguous().float()
+        pad = (C.c_float * 3)(*[-float(m) / float(s) for m, s in zip(self.mean, self.std)])
+        wins = torch.tensor(rows, dtype=torch.int32).to(dev)
+        crops = torch.empty((len(rows), 3, crop, crop), dtype=torch.float32, device=dev)
+        _lib.check(_lib.load().lseg_eval_make_crops(C.c_void_p(img.data_ptr()), C.c_void_p(crops.data_ptr()),
+                                                    C.c_void_p(wins.data_ptr()), len(rows), h, w, crop, pad,
+                                                    C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        return crops, wins
+
+    def _settings(self):
+        return (self.base_size, self.crop_size, tuple(self.mean), tuple(self.std), self.flip, tuple(self.scales),
+                self.max_batch)
+
+    @torch.no_grad()
+    def encode(self, image):
+        """The image-dependent part of `self(image, label_set)`: every crop and flip of every scale through
+        `net.encode_image`, in the batches the fused path uses. `self(encoded, label_set)` / `.predict(encoded,
+        label_set)` then run only the label-dependent tails and the canvas / resize-add glue, and return what they return
+        for the image, bit for bit. Holds one pixel embedding per network input: 36 of 62.7 MB each (2.3 GB) for a
+        683x512 image at the default scales."""
+        if not callable(getattr(self.net, "encode_image", None)):
+            raise TypeError(f"{type(self.net).__name__} has no encode_image: the evaluator cannot store its image path")
+        if self.fused is False or not image.is_cuda:
+            raise TypeError("encode() runs the fused device path: fused=False and CPU images have no stored embeddings")
+        batch, _, h, w = image.shape
+        assert batch == 1, "only single image is supported for evaluation (additional_utils/models.py:62)"
+        with torch.cuda.device(image.device):
+            _, rows, _ = self._windows(h, w)
+            crops, _ = self._crops(image, rows)
+            embs = [self.net.encode_image(crops[i:i + self.max_batch]) for i in range(0, len(rows), self.max_batch)]
+        return EncodedImage(embs, (h, w), image.device, self._settings())
+
     @torch.no_grad()
     def _forward_fused(self, image, label_set):
         import ctypes as C
         from . import _lib
         lib = _lib.load()
         dev = image.device
-        _, _, h, w = image.shape
         crop = self.crop_size
-        img = image[0].contiguous().float()
-        pad = (C.c_float * 3)(*[-float(m) / float(s) for m, s in zip(self.mean, self.std)])
         per = 2 if self.flip else 1
 
         def stream():
             return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
         with torch.cuda.device(dev):
-            # every network input of every scale, built by ONE launch, and evaluated in fixed-size batches (the engine
-            # caches one launch plan per batch shape: per-scale batches of 2, 2, 8, 12, ... would rebuild it every time)
-            geo = [self._geometry(h, w, scale) for scale in self.scales]
-            rows, first = [], []
-            for g in geo:
-                first.append(len(rows))
-                for (h0, w0) in g["origins"]:
-                    rows.append([g["height"], g["width"], h0, w0, 0, len(rows)])
-                    if self.flip:
-                        rows.append([g["height"], g["width"], h0, w0, 1, len(rows)])
-            wins = torch.tensor(rows, dtype=torch.int32).to(dev)
-            crops = torch.empty((len(rows), 3, crop, crop), dtype=torch.float32, device=dev)
-            _lib.check(lib.lseg_eval_make_crops(C.c_void_p(img.data_ptr()), C.c_void_p(crops.data_ptr()),
-                                                C.c_void_p(wins.data_ptr()), len(rows), h, w, crop, pad, stream()))
+            if isinstance(image, EncodedImage):
+                if image.settings != self._settings():
+                    raise ValueError("EncodedImage was encoded by an evaluator with other sizes, scales or batching")
+                h, w = image.size
+                geo, rows, first = self._windows(h, w)
+                wins = torch.tensor(rows, dtype=torch.int32).to(dev)
+                inputs = image.batches
+            else:
+                _, _, h, w = image.shape
+                geo, rows, first = self._windows(h, w)
+                # evaluated in fixed-size batches (the engine caches one launch plan per batch shape: per-scale batches
+                # of 2, 2, 8, 12, ... would rebuild it every time)
+                crops, wins = self._crops(image, rows)
+                inputs = [crops[i:i + self.max_batch] for i in range(0, len(rows), self.max_batch)]
             outs = None
             direct = getattr(self.net, "supports_out", False)  # LSegNet writes straight into the output batch
-            for i in range(0, len(rows), self.max_batch):
+            for i, x in zip(range(0, len(rows), self.max_batch), inputs):
                 if direct and outs is not None:
-                    self.net(crops[i:i + self.max_batch], label_set, out=outs[i:i + self.max_batch])
+                    self.net(x, label_set, out=outs[i:i + self.max_batch])
                     continue
-                o = self.net(crops[i:i + self.max_batch], label_set).float()
+                o = self.net(x, label_set).float()
                 if outs is None:
                     outs = torch.empty((len(rows),) + tuple(o.shape[1:]), dtype=torch.float32, device=dev)
                 outs[i:i + o.shape[0]] = o
@@ -204,6 +253,10 @@ class MultiScaleEvaluator:
 
     @torch.no_grad()
     def forward(self, image, label_set=""):
+        if isinstance(image, EncodedImage):
+            if self.fused is False:
+                raise TypeError("an EncodedImage is evaluated by the fused device path; this evaluator has fused=False")
+            return self._forward_fused(image, label_set)
         batch, _, h, w = image.shape
         assert batch == 1, "only single image is supported for evaluation (additional_utils/models.py:62)"
         fused = image.is_cuda if self.fused is None else self.fused
@@ -247,3 +300,14 @@ class MultiScaleEvaluator:
         h, w = image.shape[2:]
         n = sum(len(self._geometry(h, w, s)["origins"]) for s in self.scales)
         return (n * (2 if self.flip else 1), n * (2 if self.flip else 1))
+
+
+class EncodedImage:
+    """`MultiScaleEvaluator.encode(image)`: the pixel embeddings of every network input of one image (one
+    PixelEmbedding per batch of the fused path), the image size and the evaluator settings they were made with."""
+
+    def __init__(self, batches, size, device, settings):
+        self.batches = batches
+        self.size = tuple(size)
+        self.device = device
+        self.settings = settings

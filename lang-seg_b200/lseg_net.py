@@ -2,7 +2,8 @@
 
 Mirrors the reference interface for the hot path (SURVEY.md section 8(b)):
   * constructor signatures of modules/models/lseg_net.py:208-226 and lseg_net_zs.py:219-239;
-  * `forward(x, labelset='')` (lseg_net.py:160) / `forward(x, class_info)` (lseg_net_zs.py:177);
+  * `forward(x, labelset='')` (lseg_net.py:160) / `forward(x, class_info)` (lseg_net_zs.py:177); beyond the reference,
+    `x` may be a PixelEmbedding from `encode_image(x)`: only the label-dependent tail then runs, with the same result;
   * attributes the callers touch: `.pretrained.model.patch_embed.img_size` (lseg_module.py:86-89),
     `.scratch`, `.clip_pretrained` (with `.encode_text`), `.labels`, `.text`, `.crop_size`, `.out_c`,
     `.arch_option`, `.logit_scale`;
@@ -12,6 +13,7 @@ Mirrors the reference interface for the hot path (SURVEY.md section 8(b)):
 The torch sub-modules below are parameter holders only (they give the reference's names, shapes and
 default inits); no torch op runs in forward. There is no CPU path: a non-CUDA input raises.
 """
+import itertools
 import threading
 import weakref
 from collections import OrderedDict
@@ -175,6 +177,64 @@ class _ClipTextHolder(nn.Module):
 
 _IGNORED_PREFIXES = ("clip_pretrained.visual.", "pretrained.model.head.", "pretrained.model.pre_logits.")
 
+_WEIGHTS_GENERATION = itertools.count(1)  # process-wide: an embedding of another net never matches either
+
+
+class PixelEmbedding:
+    """LSeg's pixel embedding of B images, as `LSegNet.encode_image` returns it: the output of the image path (trunk,
+    decoder, head1; lseg_net.py:166-185) that every label set is then queried against. Pass it wherever the net takes
+    `x` — forward / predict / update_metric run only the label-dependent tail on it and return what they return for the
+    images themselves, bit for bit.
+
+    Holds the engine's own pair (include/lseg_b200.h): `emb` fp16 [B,H/2,W/2,out_c] un-normalised rows and `sumsq` fp32
+    [B,H/2,W/2,out_c/32] partial squared norms. `features()` gives the reference's normalised image_features. 62.7 MB
+    per 480x480 image (out_c 512)."""
+
+    def __init__(self, emb, sumsq, size, backbone, out_c, generation):
+        self.emb = emb
+        self.sumsq = sumsq
+        self.size = tuple(size)  # (H, W) of the encoded images
+        self.backbone = backbone
+        self.out_c = out_c
+        self.generation = generation
+
+    @property
+    def device(self):
+        return self.emb.device
+
+    @property
+    def shape(self):
+        """(B, 3, H, W): the shape of the images it encodes, where code reads x.shape."""
+        return (self.emb.shape[0], 3) + self.size
+
+    def __len__(self):
+        return self.emb.shape[0]
+
+    def __getitem__(self, idx):
+        if not isinstance(idx, slice) or idx.step not in (None, 1):
+            raise TypeError("PixelEmbedding supports contiguous batch slices emb[i:j]")
+        return PixelEmbedding(self.emb[idx], self.sumsq[idx], self.size, self.backbone, self.out_c, self.generation)
+
+    @staticmethod
+    def cat(embs):
+        """Concatenate along the batch: same net, weights and image size."""
+        embs = list(embs)
+        if not embs:
+            raise ValueError("PixelEmbedding.cat of nothing")
+        e0 = embs[0]
+        for e in embs[1:]:
+            if (e.size, e.backbone, e.out_c, e.generation, e.device) != (e0.size, e0.backbone, e0.out_c, e0.generation,
+                                                                         e0.device):
+                raise ValueError("PixelEmbedding.cat: embeddings of different image sizes, nets, weights or devices")
+        return PixelEmbedding(torch.cat([e.emb for e in embs]), torch.cat([e.sumsq for e in embs]), e0.size, e0.backbone,
+                              e0.out_c, e0.generation)
+
+    def features(self):
+        """The reference's normalised per-pixel embedding image_features (lseg_net.py:187-191, before `@ text.t()`) as
+        fp32 [B, out_c, H/2, W/2]."""
+        from .engine import embedding_features
+        return embedding_features(self.emb, self.sumsq)
+
 
 class _LSegBase(nn.Module):
     def _init_common(self, **kwargs):
@@ -210,7 +270,8 @@ class _LSegBase(nn.Module):
         self.logit_scale = torch.tensor(reference_logit_scale())
         self.clip_pretrained._owner = weakref.ref(self)
         self._install_load_hooks()
-        self._shared = {"engines": {}, "text_cache": {}, "lock": threading.Lock(), "master": weakref.ref(self)}
+        self._shared = {"engines": {}, "text_cache": {}, "lock": threading.Lock(), "master": weakref.ref(self),
+                        "generation": next(_WEIGHTS_GENERATION)}
         self._fast_init()
 
     def _fast_init(self):
@@ -260,6 +321,7 @@ class _LSegBase(nn.Module):
             with self._shared["lock"]:
                 self._shared["engines"].clear()
                 self._shared["text_cache"].clear()
+                self._shared["generation"] = next(_WEIGHTS_GENERATION)  # embeddings encoded so far are stale
 
     def refresh(self):
         """Re-pack weights after in-place parameter edits."""
@@ -325,6 +387,27 @@ class _LSegBase(nn.Module):
             cache[key] = feats
         return feats
 
+    @torch.no_grad()
+    def encode_image(self, x):
+        """The image path of forward (trunk, decoder, head1; lseg_net.py:166-185) of x fp32 [B,3,H,W] -> a
+        PixelEmbedding to pass to forward / predict / update_metric in place of x, with any label set."""
+        self._check_eval()
+        engine = self._engine_for(x.device)
+        emb, sumsq = engine.encode_image(x.float())
+        return PixelEmbedding(emb, sumsq, x.shape[2:], self.backbone, self.out_c, self._shared["generation"])
+
+    def _embedding_engine(self, emb):
+        """The engine that queries `emb`, after checking that this net's current weights produced it."""
+        if emb.backbone != self.backbone or emb.out_c != self.out_c:
+            raise ValueError(f"embedding of backbone {emb.backbone!r} (out_c {emb.out_c}); this net is {self.backbone!r} "
+                             f"(out_c {self.out_c})")
+        if emb.generation != self._shared["generation"]:
+            raise ValueError("embedding was encoded by another net, or with weights that have changed since "
+                             "(load_state_dict / refresh / .to()): encode the images again")
+        if emb.device.type != "cuda":
+            raise ValueError(f"embedding is on {emb.device}; lseg_b200 runs on CUDA only")
+        return self._engine_for(emb.device)
+
     def _check_eval(self):
         if self.training:
             raise NotImplementedError("lseg_b200.LSegNet is inference-only (BatchNorm running stats, no autograd); "
@@ -360,6 +443,14 @@ class LSegNet(_LSegBase):
             text = self.text
         else:
             text = tokenize(labelset)
+        if isinstance(x, PixelEmbedding):
+            engine = self._embedding_engine(x)
+            feats = self._text_features(engine, text)
+            b, (h, w), k = len(x), x.size, text.shape[0]
+            if out is None:
+                out = torch.empty((b, k, h, w), dtype=torch.float32, device=x.device)
+            engine.query(x.emb, x.sumsq, feats, k, logits=out)
+            return out
         engine = self._engine_for(x.device)
         feats = self._text_features(engine, text)
         if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or
@@ -381,6 +472,11 @@ class LSegNet(_LSegBase):
         never written (SURVEY.md 8(f) row 2)."""
         self._check_eval()
         text = self._labelset_tokens(labelset)
+        if isinstance(x, PixelEmbedding):
+            engine = self._embedding_engine(x)
+            mask = torch.empty((len(x),) + x.size, dtype=torch.int64, device=x.device)
+            engine.query(x.emb, x.sumsq, self._text_features(engine, text), text.shape[0], mask=mask)
+            return mask
         engine = self._engine_for(x.device)
         feats = self._text_features(engine, text)
         return engine.forward_argmax(x.float(), feats, text.shape[0])
@@ -393,11 +489,15 @@ class LSegNet(_LSegBase):
         from .metrics import _as_target
         self._check_eval()
         text = self._labelset_tokens(labelset)
-        engine = self._engine_for(x.device)
+        emb = x if isinstance(x, PixelEmbedding) else None
+        engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
         feats = self._text_features(engine, text)
         stats = metric._buffer(x.device)
         t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
-        engine.forward_stats(x.float(), feats, text.shape[0], t, stats, metric.nclass)
+        if emb is not None:
+            engine.query(emb.emb, emb.sumsq, feats, text.shape[0], target=t, stats=stats, nclass=metric.nclass)
+        else:
+            engine.forward_stats(x.float(), feats, text.shape[0], t, stats, metric.nclass)
 
 
 class LSegNetZS(_LSegBase):
@@ -442,6 +542,12 @@ class LSegNetZS(_LSegBase):
     @torch.no_grad()
     def forward(self, x, class_info):
         self._check_eval()
+        if isinstance(x, PixelEmbedding):
+            engine = self._embedding_engine(x)
+            out = torch.empty((len(x), 2) + x.size, dtype=torch.float32, device=x.device)
+            engine.query(x.emb, x.sumsq, self._image_text(engine, class_info, x.device), 2, text_image_stride=2,
+                         logits=out)
+            return out
         engine = self._engine_for(x.device)
         return engine.forward(x.float(), self._image_text(engine, class_info, x.device), 2, text_image_stride=2)
 
@@ -454,6 +560,12 @@ class LSegNetZS(_LSegBase):
     def predict(self, x, class_info):
         """argmax over the ['others', name] pair per pixel (test_lseg_zs.py:301), fused on the device."""
         self._check_eval()
+        if isinstance(x, PixelEmbedding):
+            engine = self._embedding_engine(x)
+            mask = torch.empty((len(x),) + x.size, dtype=torch.int64, device=x.device)
+            engine.query(x.emb, x.sumsq, self._image_text(engine, class_info, x.device), 2, text_image_stride=2,
+                         mask=mask)
+            return mask
         engine = self._engine_for(x.device)
         return engine.forward_argmax(x.float(), self._image_text(engine, class_info, x.device), 2, text_image_stride=2)
 
@@ -465,12 +577,17 @@ class LSegNetZS(_LSegBase):
         synchronisation is forward()'s class_info range check. A padded input takes a target padded with -1."""
         from .metrics import _as_target, _fewshot_target
         self._check_eval()
-        engine = self._engine_for(x.device)
+        emb = x if isinstance(x, PixelEmbedding) else None
+        engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
         text = self._image_text(engine, class_info, x.device)
         t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
         t = _fewshot_target(t, query_ignore_idx)
         group = torch.as_tensor(class_info).to(x.device)
-        engine.forward_stats(x.float(), text, 2, t, meter.stats, 2, group=group, text_image_stride=2)
+        if emb is not None:
+            engine.query(emb.emb, emb.sumsq, text, 2, text_image_stride=2, target=t, stats=meter.stats, nclass=2,
+                         group=group)
+        else:
+            engine.forward_stats(x.float(), text, 2, t, meter.stats, 2, group=group, text_image_stride=2)
 
 
 class LSegRNNetZS(LSegNetZS):

@@ -445,6 +445,38 @@ int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, i
                const long long* target, const int* group, int nclass, int G, long long* stats,
                void* stream);
 
+/* Ragged batch: every image brings its own label set (open-vocabulary serving: one prompt per request, batched for
+ * throughput). Image b's k[b] labels are rows text_row[b] .. text_row[b] + k[b] - 1 of ONE packed text operand `text`
+ * (fp16 [text_rows, out_c], L2-normalised rows as lseg_encode_text writes them, 16-byte aligned); blocks may overlap or
+ * be shared. Image b's pixels meet only its own labels: the pixel x text GEMM is one launch over the tiles of each
+ * image's own pixel rows x its own text rows, not over the union of the label sets. Outputs are packed by image, with
+ * koff[b] = k[0] + ... + k[b-1]:
+ *   logits  fp32 [sum k, H, W]  image b's logits are planes koff[b] .. koff[b] + k[b] - 1
+ *   mask    int64 [B, H, W]     mask[b] indexes image b's own labels (first maximal label, as lseg_forward_argmax)
+ * each nullable, at least one requested. Image b's planes and mask equal, bit for bit, what lseg_forward /
+ * lseg_forward_argmax write for that image alone (B = 1) with its k[b] rows as the label set. k and text_row are HOST
+ * arrays of B ints (the planner needs the tile counts; nothing is read back from the device). Rules, each checked and
+ * rejected by name before the first launch: 1 <= B <= 64 images (the per-image tables travel in kernel parameters),
+ * k[b] >= 1, 0 <= text_row[b] and text_row[b] + k[b] <= text_rows, sum k <= 65535, H and W positive multiples of 32,
+ * W <= 1024. arch_option 1 / 2 runs the head blocks once per image (their channel max is over the image's own labels).
+ * Stream contract as for the other engine calls: everything is enqueued on `stream`; the host arrays may be reused as
+ * soon as the call returns. */
+int lseg_forward_ragged(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int text_rows,
+                        const int* text_row, const int* k, float* logits, long long* mask, void* stream);
+
+/* lseg_forward_ragged's label-dependent tail on an embedding pair (lseg_encode_image) of B images of H x W; same tables,
+ * outputs and rules. Allocates only the tail's buffers, like lseg_query. */
+int lseg_query_ragged(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W, const void* text,
+                      int text_rows, const int* text_row, const int* k, float* logits, long long* mask, void* stream);
+
+/* Stage op: the ragged pixel x text GEMM alone. a fp16 [B*P, C] row-major (P pixels per image, a multiple of 128; C a
+ * multiple of 64), text / text_rows / text_row / k as in lseg_forward_ragged -> out fp16 [sum k, P]: plane koff[b] + j =
+ * image b's pixel rows times its text row text_row[b] + j, scaled per row by row_scale * rsqrt(sum of the row's
+ * row_sumsq_parts entries of row_sumsq fp32 [B*P, parts]) when row_sumsq is non-NULL (the engine's normalisation),
+ * unscaled when it is NULL. Only those planes are written. Enqueued on `stream`. */
+int lseg_gemm_ragged(const void* a, const float* row_sumsq, int row_sumsq_parts, float row_scale, int B, int P, int C,
+                     const void* text, int text_rows, const int* text_row, const int* k, void* out, void* stream);
+
 /* The reference's normalised pixel embedding image_features (lseg_net.py:187-191) from an embedding pair of B images
  * with an h x w grid: out fp32 NCHW [B, C, h, w] = emb * rsqrt(sum of the C/32 partials, in index order). C in
  * {512, 768}; h*w a multiple of 4; emb and out 16-byte aligned. No engine needed. */

@@ -98,6 +98,7 @@ SYMBOLS = [
     "lseg_eval_make_crops", "lseg_eval_canvas", "lseg_eval_resize_add", "lseg_preprocess",
     "lseg_seg_stats_scores", "lseg_seg_stats_mask", "lseg_forward_segstats",
     "lseg_encode_image", "lseg_query", "lseg_embedding_features",
+    "lseg_forward_ragged", "lseg_query_ragged", "lseg_gemm_ragged",
 ]
 
 _lib = None
@@ -204,6 +205,11 @@ def load(build_if_missing=True):
                                C.c_void_p, C.c_void_p]
     lib.lseg_embedding_features.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                             C.c_void_p]
+    _ragged = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.lseg_forward_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + _ragged
+    lib.lseg_query_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int] + _ragged
+    lib.lseg_gemm_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
     lib.lseg_last_launch_count.argtypes = [C.c_void_p]
     lib.lseg_forward_profiled.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                           C.c_longlong, C.c_void_p, C.c_void_p, C.POINTER(C.c_float),

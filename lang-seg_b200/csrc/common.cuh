@@ -54,6 +54,9 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank
 // pass, instead of re-polling every ~100 cycles and stealing issue slots from the compute warps that
 // share its SM sub-partition.
 constexpr uint32_t kTryWaitHintNs = 20000;
+// Most images in one ragged call (every image its own label set): the per-image tables of the pixel x text GEMM and of
+// the argmax output stage travel in kernel parameters.
+constexpr int kRaggedMaxImages = 64;
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(

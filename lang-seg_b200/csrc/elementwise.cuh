@@ -806,11 +806,12 @@ static inline int launch_upsample2x_nchw_bg(const __half* x, float* y, long long
 // is flushed once per block; the mask store becomes optional (mask may be nullptr).
 // ------------------------------------------------------------------------------------------
 constexpr int kArgJ = 16;  // outputs per lane per pass (Wo <= 512 in one pass)
+// plane0: index of the image's first low-res plane in lr (b * K for one label set; its K planes follow it)
 template <typename TIn, bool kStats>
 __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr, long long* __restrict__ mask, int K, int H,
                                                       int W, int b, int oy, int lane, float (*line)[kUpMaxW],
                                                       const SegStatsArgs& st, int* hist, unsigned long long* grow,
-                                                      int& labeled, int& correct) {
+                                                      int& labeled, int& correct, long long plane0) {
   const int Ho = 2 * H, Wo = 2 * W;
   const float sh = (Ho > 1) ? static_cast<float>(H - 1) / (Ho - 1) : 0.f;
   const float sw = (Wo > 1) ? static_cast<float>(W - 1) / (Wo - 1) : 0.f;
@@ -819,7 +820,7 @@ __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr
   const int y1 = min(y0 + 1, H - 1);
   const float ly = fy - y0, hy = 1.f - ly;
   const long long plane_sz = static_cast<long long>(H) * W;
-  const TIn* img = lr + static_cast<long long>(b) * K * plane_sz;
+  const TIn* img = lr + plane0 * plane_sz;
   const long long row_off = (static_cast<long long>(b) * Ho + oy) * Wo;
   for (int ox0 = 0; ox0 < Wo; ox0 += 32 * kArgJ) {
     int xa[kArgJ], xb[kArgJ];
@@ -901,13 +902,36 @@ __global__ void __launch_bounds__(256) upsample2x_argmax_kernel(const TIn* __res
     seg_block_begin(hist, st.nclass);
     int labeled = 0, correct = 0;
     if (oy < 2 * H)  // warps past the last row still take part in the block's flush
-      upsample2x_argmax_row<TIn, true>(lr, mask, K, H, W, b, oy, lane, line[warp], st, hist, grow, labeled, correct);
+      upsample2x_argmax_row<TIn, true>(lr, mask, K, H, W, b, oy, lane, line[warp], st, hist, grow, labeled, correct,
+                                       static_cast<long long>(b) * K);
     if (grow) seg_block_finish(hist, grow, st.nclass, labeled, correct);
   } else {
     if (oy >= 2 * H) return;  // warp-uniform
     int unused = 0;
-    upsample2x_argmax_row<TIn, false>(lr, mask, K, H, W, b, oy, lane, line[warp], st, nullptr, nullptr, unused, unused);
+    upsample2x_argmax_row<TIn, false>(lr, mask, K, H, W, b, oy, lane, line[warp], st, nullptr, nullptr, unused, unused,
+                                      static_cast<long long>(b) * K);
   }
+}
+// Ragged batch (every image its own label set): image b's k[b] low-res planes start at plane koff[b] of the packed
+// [sum k, H, W] logits, and mask[b] indexes image b's own labels. The same row routine as upsample2x_argmax_kernel, so
+// each image's mask is bit-identical to a one-image call with its label set. The table travels in the parameters.
+struct RaggedPlanes {
+  int k[kRaggedMaxImages];
+  int koff[kRaggedMaxImages];
+};
+template <typename TIn>
+__global__ void __launch_bounds__(256) upsample2x_argmax_ragged_kernel(const TIn* __restrict__ lr, long long* __restrict__ mask,
+                                                                       int H, int W, const __grid_constant__ RaggedPlanes rp) {
+  griddep_launch_dependents();
+  griddep_wait();
+  __shared__ __align__(16) float line[8][2][kUpMaxW];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.y;
+  const int oy = blockIdx.x * 8 + warp;
+  if (oy >= 2 * H) return;  // warp-uniform
+  int unused = 0;
+  upsample2x_argmax_row<TIn, false>(lr, mask, rp.k[b], H, W, b, oy, lane, line[warp], SegStatsArgs{}, nullptr, nullptr,
+                                    unused, unused, rp.koff[b]);
 }
 static inline int check_upsample2x_argmax(int B, int K, int H, int W) {
   if (W % 8 != 0 || W > kUpMaxW || B > 65535 || K <= 0) {
@@ -921,6 +945,17 @@ static inline int launch_upsample2x_argmax(const TIn* lr, long long* mask, int B
   if (check_upsample2x_argmax(B, K, H, W)) return -1;
   launch_pdl(upsample2x_argmax_kernel<TIn, false>, dim3((2 * H + 7) / 8, B), dim3(256), 0, s, lr, mask, K, H, W,
              SegStatsArgs{});
+  LSEG_LAUNCH_CHECK();
+}
+template <typename TIn>
+static inline int launch_upsample2x_argmax_ragged(const TIn* lr, long long* mask, int B, const RaggedPlanes& rp, int H, int W,
+                                                  cudaStream_t s) {
+  if (W % 8 != 0 || W > kUpMaxW || B < 1 || B > kRaggedMaxImages) {
+    set_error("upsample2x_argmax_ragged: needs W %% 8 == 0, W <= %d, 1 <= B <= %d (W=%d B=%d)", kUpMaxW, kRaggedMaxImages,
+              W, B);
+    return -1;
+  }
+  launch_pdl(upsample2x_argmax_ragged_kernel<TIn>, dim3((2 * H + 7) / 8, B), dim3(256), 0, s, lr, mask, H, W, rp);
   LSEG_LAUNCH_CHECK();
 }
 // The same output stage with the metric counters of `st` (mask optional): dynamic shared memory holds the block

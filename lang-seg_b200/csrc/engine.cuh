@@ -27,6 +27,11 @@ struct CallCtx {
                          // fp16 matmul, lseg_net.py:194-196) instead of the plan's own buffer; may be PEER memory — the
                          // pixel x text GEMM then stores straight into another GPU's gather buffer over NVLink
   const SegStatsArgs* seg = nullptr;  // optional metric counters, fused with the argmax output stage (out_mask optional)
+  // ragged batch (lseg_forward_ragged / lseg_query_ragged): image b's rag_k[b] labels are rows rag_text_row[b] .. of
+  // `text` (rag_text_rows readable rows); K is then the sum of rag_k, and the logits / low-res planes are packed by image
+  const int* rag_k = nullptr;
+  const int* rag_text_row = nullptr;
+  int rag_text_rows = 0;
 };
 using StepFn = std::function<int(const CallCtx&, cudaStream_t)>;
 enum StepKind { KIND_EW = 0, KIND_GEMM = 1, KIND_MHSA = 2, KIND_LN = 3, KIND_MEMSET = 4 };
@@ -107,7 +112,7 @@ struct TailWs {
   float* head_cmax = nullptr;              // [B,h,w]
   size_t head_cap_k = 0;
   // pixel x text GEMM plans (host-encoded tensor maps) keyed by (text pointer, K, per-image stride, output pointer,
-  // embedding pointers)
+  // embedding pointers, and for a ragged batch its text row count and k / text_row vectors)
   struct CorrKey {
     const void* text;
     int K;
@@ -115,8 +120,9 @@ struct TailWs {
     const void* out;
     const void* emb;
     const void* sumsq;
+    std::vector<int> rag;
     bool operator<(const CorrKey& o) const {
-      return std::tie(text, K, stride, out, emb, sumsq) < std::tie(o.text, o.K, o.stride, o.out, o.emb, o.sumsq);
+      return std::tie(text, K, stride, out, emb, sumsq, rag) < std::tie(o.text, o.K, o.stride, o.out, o.emb, o.sumsq, o.rag);
     }
   };
   std::map<CorrKey, std::vector<std::pair<GemmPlan, double>>> corr;
@@ -923,7 +929,9 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
     set_error("lseg_forward_lowres: the fp16 low-res logits are not the network output when arch_option is %d", arch);
     return -1;
   }
-  TailWs* t = tail_ws(eng, B, H, W, ctx.K, !ctx.out_lr, stream);
+  const bool ragged = ctx.rag_k != nullptr;
+  // a ragged batch packs sum(k) = ctx.K planes: the per-image workspaces hold B * ceil(sum / B) >= sum planes
+  TailWs* t = tail_ws(eng, B, H, W, ragged ? (ctx.K + B - 1) / B : ctx.K, !ctx.out_lr, stream);
   if (!t) return -1;
   const int h2 = H / 2, w2 = W / 2;
   const long long P = static_cast<long long>(h2) * w2;
@@ -936,10 +944,40 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
   // image's block (nchw_group), the other columns are computed and dropped. For K = 2 the N tile is 128 wide anyway,
   // so this costs the same tile as one image's block and replaces B launches by one. Falls back to one launch per
   // image when B*stride exceeds one 256-column tile.
+  // Ragged batch (every image its own label set): ONE launch of the ragged kernel, whose work list holds only the tiles of
+  // each image's own pixel rows x its own text rows; image b's columns land in planes koff[b] .. of the packed output.
   {
-    TailWs::CorrKey key{ctx.text, ctx.K, ctx.text_image_stride, lr, emb, sumsq};
+    TailWs::CorrKey key{ctx.text, ctx.K, ctx.text_image_stride, lr, emb, sumsq, {}};
+    if (ragged) {
+      key.rag.assign(1, ctx.rag_text_rows);
+      key.rag.insert(key.rag.end(), ctx.rag_k, ctx.rag_k + B);
+      key.rag.insert(key.rag.end(), ctx.rag_text_row, ctx.rag_text_row + B);
+    }
     auto it = t->corr.find(key);
-    if (it == t->corr.end()) {
+    if (it == t->corr.end() && ragged) {
+      if (t->corr.size() > 16) t->corr.clear();
+      const int OC = eng->w.out_c;
+      GemmDesc d;
+      memset(&d, 0, sizeof(d));
+      d.a = emb;
+      d.lda = OC;
+      d.a_rows = static_cast<int>(B * P);
+      d.w = ctx.text;
+      d.w_rows = ctx.rag_text_rows;
+      d.M = static_cast<int>(B * P);
+      d.K = OC;
+      d.e = epi_none();
+      d.e.out_f16 = lr;
+      d.e.nchw_p = static_cast<int>(P);
+      d.e.row_sumsq = sumsq;
+      d.e.row_sumsq_parts = OC / 32;
+      d.e.row_scale = eng->w.logit_scale;
+      GemmPlan gp;
+      if (gemm_plan_ragged(d, B, ctx.rag_k, ctx.rag_text_row, &gp)) return -1;
+      std::vector<std::pair<GemmPlan, double>> plans;
+      plans.emplace_back(gp, 2.0 * P * ctx.K * static_cast<double>(OC));
+      it = t->corr.emplace(key, std::move(plans)).first;
+    } else if (it == t->corr.end()) {
       if (t->corr.size() > 16) t->corr.clear();
       std::vector<std::pair<GemmPlan, double>> plans;
       const long long stride = ctx.text_image_stride;
@@ -989,6 +1027,23 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
     for (int dpt = 0; dpt < depth; ++dpt) {
       const int act = (dpt + 1 < depth) ? eng->w.head_act : HEAD_ACT_NONE;
       float* dst = t->head_ws[dpt & 1];
+      if (ragged) {  // the channel max runs over each image's own labels: one launch_head_block per image
+        long long koff = 0;
+        for (int b = 0; b < B; ++b) {
+          const long long o = koff * P;
+          float* cm = t->head_cmax + b * P;
+          const int kb = ctx.rag_k[b];
+          int rc = (dpt == 0) ? launch_head_block(lr + o, cm, dst + o, 1, kb, h2, w2, hw, arch, act, stream)
+                              : launch_head_block(static_cast<const float*>(t->head_ws[(dpt - 1) & 1]) + o, cm, dst + o, 1,
+                                                  kb, h2, w2, hw, arch, act, stream);
+          if (rc) return -1;
+          if (arch == 1) ++*launches;
+          if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
+          koff += kb;
+        }
+        lr32 = dst;
+        continue;
+      }
       int rc = (dpt == 0) ? launch_head_block(lr, t->head_cmax, dst, B, ctx.K, h2, w2, hw, arch, act, stream)
                           : launch_head_block(static_cast<const float*>(t->head_ws[(dpt - 1) & 1]), t->head_cmax, dst,
                                               B, ctx.K, h2, w2, hw, arch, act, stream);
@@ -1000,7 +1055,7 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
   }
   // ---- scratch.output_conv: bilinear x2, align_corners=True (lseg_net.py:203) ----
   if (ctx.out) {
-    const long long planes = static_cast<long long>(B) * ctx.K;
+    const long long planes = ragged ? ctx.K : static_cast<long long>(B) * ctx.K;
     if (lr32 ? launch_upsample2x_nchw(lr32, ctx.out, planes, h2, w2, stream)
              : launch_upsample2x_nchw(lr, ctx.out, planes, h2, w2, stream))
       return -1;
@@ -1010,6 +1065,17 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
   if (ctx.seg) {  // ... and counted into the metric rows in the same kernel
     if (lr32 ? launch_upsample2x_segstats(lr32, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream)
              : launch_upsample2x_segstats(lr, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream))
+      return -1;
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
+  } else if (ctx.out_mask && ragged) {
+    RaggedPlanes rp;
+    memset(&rp, 0, sizeof(rp));
+    for (int b = 0, koff = 0; b < B; koff += ctx.rag_k[b], ++b) {
+      rp.k[b] = ctx.rag_k[b];
+      rp.koff[b] = koff;
+    }
+    if (lr32 ? launch_upsample2x_argmax_ragged(lr32, ctx.out_mask, B, rp, h2, w2, stream)
+             : launch_upsample2x_argmax_ragged(lr, ctx.out_mask, B, rp, h2, w2, stream))
       return -1;
     if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
   } else if (ctx.out_mask) {
@@ -1143,6 +1209,40 @@ static int build_text_plan(lseg_engine* eng, int K) {
     return 0;
   });
   eng->txt = std::move(plan);
+  return 0;
+}
+
+// Rules of a ragged batch's label table, each rejected by name: image b's k[b] >= 1 labels are rows text_row[b] ..
+// text_row[b] + k[b] - 1 of a 16-byte aligned text operand with text_rows readable rows; at most kRaggedMaxImages images;
+// sum(k) <= 65535 packed planes (the output stage's grid limit). *sum_k = sum(k).
+static int check_ragged(const char* fn, int B, const void* text, int text_rows, const int* text_row, const int* k,
+                        long long* sum_k) {
+  if (!text) return set_error("%s: null text", fn), -1;
+  if (reinterpret_cast<uintptr_t>(text) % 16) return set_error("%s: text must be 16-byte aligned", fn), -1;
+  if (!text_row) return set_error("%s: null text_row", fn), -1;
+  if (!k) return set_error("%s: null k", fn), -1;
+  if (B < 1) return set_error("%s: B=%d must be positive", fn, B), -1;
+  if (B > kRaggedMaxImages) return set_error("%s: B=%d images exceed the cap of %d per call", fn, B, kRaggedMaxImages), -1;
+  if (text_rows < 1) return set_error("%s: text_rows=%d must be positive", fn, text_rows), -1;
+  long long sum = 0;
+  for (int b = 0; b < B; ++b) {
+    if (k[b] < 1) return set_error("%s: k[%d]=%d labels must be positive", fn, b, k[b]), -1;
+    if (text_row[b] < 0 || static_cast<long long>(text_row[b]) + k[b] > text_rows)
+      return set_error("%s: text_row[%d]=%d + k[%d]=%d exceeds text_rows=%d", fn, b, text_row[b], b, k[b], text_rows), -1;
+    sum += k[b];
+  }
+  if (sum > 65535) return set_error("%s: sum of k = %lld exceeds 65535", fn, sum), -1;
+  *sum_k = sum;
+  return 0;
+}
+
+// Outputs of a ragged call: logits fp32 [sum k, H, W] and / or mask int64 [B, H, W], at least one; the x2 output stage
+// reads rows of at most 2 * kUpMaxW pixels.
+static int check_ragged_outputs(const char* fn, const float* logits, const long long* mask, int W) {
+  if (!logits && !mask) return set_error("%s: no output requested (logits or mask)", fn), -1;
+  if (logits && reinterpret_cast<uintptr_t>(logits) % 16) return set_error("%s: logits must be 16-byte aligned", fn), -1;
+  if (mask && reinterpret_cast<uintptr_t>(mask) % 8) return set_error("%s: mask must be 8-byte aligned", fn), -1;
+  if (W > 2 * kUpMaxW) return set_error("%s: W=%d must be <= %d", fn, W, 2 * kUpMaxW), -1;
   return 0;
 }
 
@@ -1411,6 +1511,65 @@ int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, i
   ctx.out = logits;
   ctx.out_mask = mask;
   ctx.seg = seg ? &st : nullptr;
+  int launches = 0;
+  __half* lr = nullptr;
+  if (run_tail(e, ctx, B, H, W, static_cast<const __half*>(emb), emb_sumsq, static_cast<cudaStream_t>(stream), nullptr,
+               &launches, &lr))
+    return -1;
+  e->last_launches = launches;
+  return 0;
+}
+
+int lseg_forward_ragged(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int text_rows,
+                        const int* text_row, const int* k, float* logits, long long* mask, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_forward_ragged";
+  // every rule is checked here, before the first launch
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!x) return set_error("%s: null x", fn), -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  long long sum_k = 0;
+  if (check_ragged(fn, B, text, text_rows, text_row, k, &sum_k)) return -1;
+  if (check_ragged_outputs(fn, logits, mask, W)) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.x = x;
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = static_cast<int>(sum_k);
+  ctx.out = logits;
+  ctx.out_mask = mask;
+  ctx.rag_k = k;
+  ctx.rag_text_row = text_row;
+  ctx.rag_text_rows = text_rows;
+  return run_forward(e, ctx, B, H, W, static_cast<cudaStream_t>(stream));
+}
+
+int lseg_query_ragged(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W, const void* text,
+                      int text_rows, const int* text_row, const int* k, float* logits, long long* mask, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_query_ragged";
+  // every rule is checked here, before the first launch
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 16) return set_error("%s: emb_sumsq must be 16-byte aligned", fn), -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  long long sum_k = 0;
+  if (check_ragged(fn, B, text, text_rows, text_row, k, &sum_k)) return -1;
+  if (check_ragged_outputs(fn, logits, mask, W)) return -1;
+  if (ensure_init()) return -1;
+  LSEG_CHECK_CUDA(cudaSetDevice(e->device));
+  if (ensure_init()) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = static_cast<int>(sum_k);
+  ctx.out = logits;
+  ctx.out_mask = mask;
+  ctx.rag_k = k;
+  ctx.rag_text_row = text_row;
+  ctx.rag_text_rows = text_rows;
   int launches = 0;
   __half* lr = nullptr;
   if (run_tail(e, ctx, B, H, W, static_cast<const __half*>(emb), emb_sumsq, static_cast<cudaStream_t>(stream), nullptr,

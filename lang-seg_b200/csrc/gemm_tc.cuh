@@ -94,6 +94,64 @@ struct GemmParams {
   GemmEpi e;
 };
 
+// Ragged pixel x text product (gemm_tc_kernel RAGGED): B images, each with its own label set. Image b's P pixel rows
+// (rows b*P .. b*P + P - 1 of A, P a multiple of 128, so no tile straddles two images) meet only text rows
+// text_row[b] .. text_row[b] + k[b] - 1 of the one packed text operand (tma_b), and its k[b] columns are stored as planes
+// koff[b] .. koff[b] + k[b] - 1 of a packed fp16 [sum k, h, w] output (STORE_NCHW_T, nchw_p = P). The work list is
+// image-major, m-fastest within an image: image b owns tiles tile0[b] .. tile0[b+1] - 1, m_tiles(P) * ceil(k[b] / 128).
+// The table travels in the kernel's __grid_constant__ parameters (no host synchronisation, no device copy), so the
+// image count is capped (kRaggedMaxImages).
+struct GemmRaggedTable {
+  int n;         // images
+  int m_tiles;   // 128-row tiles per image (P / 128)
+  int tile0[kRaggedMaxImages + 1];
+  int k[kRaggedMaxImages];
+  int text_row[kRaggedMaxImages];
+  int koff[kRaggedMaxImages];
+};
+struct GemmRaggedParams : GemmParams {
+  GemmRaggedTable rt;
+};
+template <bool RAGGED> struct GemmParamsOf { using type = GemmParams; };
+template <> struct GemmParamsOf<true> { using type = GemmRaggedParams; };
+
+// Work-list entry -> (m_tile, n_tile) and the first B row of the tile. Plain lists are m-fastest over
+// num_m_tiles x num_n_tiles (CLUSTER: over pair units, the CTA of rank r takes n-tile 2 j + r); ragged lists are decoded
+// through the table (img = the image, whose label count / first output plane the epilogue needs).
+struct GemmTileCoord {
+  int m_tile, n_tile, b_row, img;
+};
+template <bool CLUSTER>
+__device__ __forceinline__ GemmTileCoord gemm_tile_coord(const GemmParams& p, int tile, int rank) {
+  GemmTileCoord c;
+  c.m_tile = tile % p.num_m_tiles;
+  c.n_tile = CLUSTER ? 2 * (tile / p.num_m_tiles) + rank : tile / p.num_m_tiles;
+  c.b_row = c.n_tile * kGemmBN;
+  c.img = 0;
+  return c;
+}
+template <bool CLUSTER>
+__device__ __forceinline__ GemmTileCoord gemm_tile_coord(const GemmRaggedParams& p, int tile, int) {
+  GemmTileCoord c;
+  int b = 0;
+  while (b + 1 < p.rt.n && tile >= p.rt.tile0[b + 1]) ++b;
+  const int local = tile - p.rt.tile0[b];
+  c.m_tile = b * p.rt.m_tiles + local % p.rt.m_tiles;
+  c.n_tile = local / p.rt.m_tiles;
+  c.b_row = p.rt.text_row[b] + c.n_tile * kGemmBN;
+  c.img = b;
+  return c;
+}
+__device__ __forceinline__ int gemm_num_units(const GemmParams& p, bool cluster) {
+  return p.num_m_tiles * (cluster ? p.num_n_tiles / 2 : p.num_n_tiles);
+}
+__device__ __forceinline__ int gemm_num_units(const GemmRaggedParams& p, bool) { return p.rt.tile0[p.rt.n]; }
+// label count / first output plane of image img (ragged epilogue); 0 for plain lists
+__device__ __forceinline__ int gemm_ragged_k(const GemmParams&, int) { return 0; }
+__device__ __forceinline__ int gemm_ragged_k(const GemmRaggedParams& p, int img) { return p.rt.k[img]; }
+__device__ __forceinline__ int gemm_ragged_koff(const GemmParams&, int) { return 0; }
+__device__ __forceinline__ int gemm_ragged_koff(const GemmRaggedParams& p, int img) { return p.rt.koff[img]; }
+
 // Debug timeline of one warp (lseg_debug_gemm_trace): stamps are dropped when w == nullptr (always, unless enabled).
 // The stamp itself is an out-of-line call so that the untraced kernel pays one predicated branch per site, not a
 // predicated copy of the stamp code.
@@ -211,9 +269,10 @@ __device__ __forceinline__ void gemm_epilogue_math(const GemmEpi& e, int N, cons
 // (zero-shot path) — a compile-time variant: as a runtime case it costs the common kernel 4 registers and 128
 // instructions (the one-label-set instantiation is instruction-for-instruction the round-1 kernel again).
 // RELU_RES: GemmEpi::relu_after_res (ResNet bottleneck output), row-major full chunks and tails alike.
-template <bool GROUPED = false, bool RELU_RES = false>
+// RAGGED: STORE_NCHW_T of one image of a ragged list — N is the image's label count and koff its first output plane.
+template <bool GROUPED = false, bool RELU_RES = false, bool RAGGED = false>
 __device__ __forceinline__ void gemm_epilogue_store(const GemmEpi& e, int N, float (&f)[32], const float4 (&res)[8],
-                                                    bool has_res, long long grow, int n0) {
+                                                    bool has_res, long long grow, int n0, int koff = 0) {
   const int nvalid = min(32, N - n0);
   if (e.store == STORE_ROWMAJOR) {
     const long long off = grow * e.ldc + n0;
@@ -315,7 +374,12 @@ __device__ __forceinline__ void gemm_epilogue_store(const GemmEpi& e, int N, flo
   } else {  // STORE_NCHW_T : out[(b*K + n)*P + p], fp16 (lanes = consecutive pixels -> coalesced)
     const int b = static_cast<int>(grow / e.nchw_p);
     const int pix = static_cast<int>(grow - static_cast<long long>(b) * e.nchw_p);
-    if constexpr (!GROUPED) {  // one label set for all images: the chunk's columns are channels n0 .. n0+31
+    if constexpr (RAGGED) {  // the image's own label set: columns n0 .. n0+31 are planes koff + n0 .. of the packed output
+      __half* op = e.out_f16 + (static_cast<long long>(koff) + n0) * e.nchw_p + pix;
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (n0 + i < N) op[static_cast<long long>(i) * e.nchw_p] = __float2half_rn(f[i]);
+    } else if constexpr (!GROUPED) {  // one label set for all images: the chunk's columns are channels n0 .. n0+31
       __half* op = e.out_f16 + (static_cast<long long>(b) * e.nchw_k + n0) * e.nchw_p + pix;
 #pragma unroll
       for (int i = 0; i < 32; ++i)
@@ -371,31 +435,35 @@ __device__ __forceinline__ void gemm_acc_ld32(const float* acc_row, int c, int r
 // this thread's row of the staged accumulators (gemm_acc_ld32), whose column 0 is output column n_base.
 // SINGLE_BUF: one 4 KB staging tile per warp instead of two (leaves the shared memory to the accumulator tile and the
 // operand ring; the warp then waits for its previous bulk store to finish reading before it refills the buffer).
-template <int EPI, bool SINGLE_BUF = false, bool GROUPED = false, bool RELU_RES = false, typename WaitFn>
+// RAGGED: the tile belongs to an image with rag_k labels whose first output plane is rag_koff (gemm_epilogue_store); its
+// column count takes the place of p.N.
+template <int EPI, bool SINGLE_BUF = false, bool GROUPED = false, bool RELU_RES = false, bool RAGGED = false,
+          typename WaitFn>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc_row, int n_base, int ncols,
                                                    int m_tile, int r, WaitFn wait_accumulator, uint8_t* stage_buf,
                                                    int& store_groups, GemmTrace& tr, bool first_k = true,
-                                                   int split_seg = 0) {
+                                                   int split_seg = 0, int rag_k = 0, int rag_koff = 0) {
   const GemmEpi& e = p.e;
   long long grow;
   const bool valid = gemm_row_map(p, m_tile, r, grow);
   // split_fixed: this segment's plane of the partial-sum workspace (split_rows is 0 otherwise)
   if constexpr (EPI == EPI_DIRECT) grow += split_seg * p.split_rows;
   if constexpr (EPI == EPI_DIRECT) {
+    const int& N = RAGGED ? rag_k : p.N;  // plain lists: p.N itself (a parameter-space operand, as before)
     // The fp32 residual of chunk c+1 is requested before chunk c is processed, and that of chunk 0 before the
     // accumulator is even ready, so the residual read latency overlaps the main loop / the previous chunk.
     const bool pre = valid && e.res_f32 && (e.store == STORE_ROWMAJOR);
     const long long bias_off =
-        (e.bias_group_rows > 0 && valid) ? (grow / e.bias_group_rows) * static_cast<long long>(p.N) : 0;
+        (e.bias_group_rows > 0 && valid) ? (grow / e.bias_group_rows) * static_cast<long long>(N) : 0;
     float4 rnext[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) rnext[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (pre && n_base + 32 <= p.N) {
+    if (pre && n_base + 32 <= N) {
       const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n_base);
 #pragma unroll
       for (int j = 0; j < 8; ++j) rnext[j] = rp[j];
     }
-    const GemmColConst cc = gemm_col_const(e, p.N, n_base, ncols, r & 31);
+    const GemmColConst cc = gemm_col_const(e, N, n_base, ncols, r & 31);
     float row_mul = 1.f;
     if (e.row_sumsq && valid) {  // deferred pixel normalisation: logit_scale / ||feature row||, once per tile
       float ss = 0.f;
@@ -408,12 +476,12 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
 #pragma unroll 1
     for (int c = 0; c < ncols / 32; ++c) {
       const int n0 = n_base + c * 32;
-      if (n0 >= p.N) break;  // warp-uniform
+      if (n0 >= N) break;  // warp-uniform
       float4 rcur[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
-      const bool has_res = pre && (n0 + 32 <= p.N);
-      if (pre && (c + 1) * 32 < ncols && n0 + 64 <= p.N) {
+      const bool has_res = pre && (n0 + 32 <= N);
+      if (pre && (c + 1) * 32 < ncols && n0 + 64 <= N) {
         const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n0 + 32);
 #pragma unroll
         for (int j = 0; j < 8; ++j) rnext[j] = rp[j];
@@ -422,13 +490,13 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
       __syncwarp();
       gemm_acc_ld32(acc_row, c, r, v);
       float f[32];
-      gemm_epilogue_math(e, p.N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
+      gemm_epilogue_math(e, N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
       if (valid) {
         if (e.row_sumsq) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) f[i] *= row_mul;
         }
-        gemm_epilogue_store<GROUPED, RELU_RES>(e, p.N, f, rcur, has_res, grow, n0);
+        gemm_epilogue_store<GROUPED, RELU_RES, RAGGED>(e, N, f, rcur, has_res, grow, n0, rag_koff);
       }
     }
   } else {
@@ -577,9 +645,16 @@ __device__ __forceinline__ void gemm_stage_half(float* acc_half, float (&acc)[64
 // own CTA and on the peer's (count 8). The two lists have the same k ranges, so the ring stage / parity sequence and the
 // ping-pong turn order are the same in both CTAs. Every output element sums the same k16 chunks in the same order through
 // the same instruction as without clusters: results are bit-identical. Needs an even n-tile count and no stream-K split.
-template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false, bool CLUSTER = false>
-__global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+// RAGGED: the parameters carry a per-image problem table (GemmRaggedTable) and the work list is decoded through it; the
+// K loop and the epilogue arithmetic are the plain NCHW-T kernel's, so image b's logits are bit-identical to those of a
+// one-image call with its own label set (an accumulator column does not depend on its neighbours). Unclustered.
+template <int EPI, bool FIXED_SPLIT = false, bool GROUPED = false, bool RELU_RES = false, bool CLUSTER = false,
+          bool RAGGED = false>
+__global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1)
+    gemm_tc_kernel(const __grid_constant__ typename GemmParamsOf<RAGGED>::type p) {
   static_assert(!RELU_RES || (EPI == EPI_DIRECT && !FIXED_SPLIT && !GROUPED), "relu-after-residual: plain register-direct");
+  static_assert(!RAGGED || (EPI == EPI_DIRECT && !FIXED_SPLIT && !GROUPED && !RELU_RES && !CLUSTER),
+                "ragged pixel x text: NCHW-T store, register-direct, unclustered");
   static_assert(!FIXED_SPLIT || EPI == EPI_DIRECT, "split-K partials leave through the register-direct epilogue");
   static_assert(!GROUPED || (EPI == EPI_DIRECT && !FIXED_SPLIT), "per-image column blocks: NCHW-T store, register-direct");
   using Cfg = GemmCfg<EPI>;
@@ -615,8 +690,8 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     __syncthreads();
   griddep_wait();  // everything above overlapped the previous kernel's tail; operands / outputs are touched below
 
-  // CLUSTER: the list is over pair units (num_n_tiles is even)
-  const int num_tiles = p.num_m_tiles * (CLUSTER ? p.num_n_tiles / 2 : p.num_n_tiles);
+  // CLUSTER: the list is over pair units (num_n_tiles is even); RAGGED: the table's tile count
+  const int num_tiles = gemm_num_units(p, CLUSTER);
 
   // Work schedule of this CTA. Default: whole tiles cta, cta + G, ... . split_k (in-place residual GEMMs only, whose
   // epilogue is a reduce-add and therefore composes over partial sums): the (tile, k-chunk) units are dealt out evenly,
@@ -681,8 +756,9 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     Sched sc = make_sched();
     int tile, k_begin, k_end;
     while ((!CLUSTER || warp == 0) && sc.next(tile, k_begin, k_end)) {
-      const int m_tile = tile % p.num_m_tiles;
-      const int n0 = (CLUSTER ? 2 * (tile / p.num_m_tiles) + rank : tile / p.num_m_tiles) * kGemmBN;
+      const GemmTileCoord tc = gemm_tile_coord<CLUSTER>(p, tile, rank);
+      const int m_tile = tc.m_tile;
+      const int n0 = tc.b_row;
       int cb = 0, ch0 = 0, cw0 = 0;
       if (p.conv) {
         const int per_img = p.tiles_h * p.tiles_w;
@@ -760,8 +836,10 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
     int tile, k_begin, k_end;
     bool more = sc.next(tile, k_begin, k_end);
     for (int idx = 0; more; ++idx) {
-      const int m_tile = tile % p.num_m_tiles;
-      const int n_tile = CLUSTER ? 2 * (tile / p.num_m_tiles) + rank : tile / p.num_m_tiles;
+      const GemmTileCoord tc = gemm_tile_coord<CLUSTER>(p, tile, rank);
+      const int m_tile = tc.m_tile;
+      const int n_tile = tc.n_tile;
+      const int img = tc.img;
       const int kb = k_begin, ke = k_end;
       const int seg = FIXED_SPLIT ? sc.seg : 0;
       more = sc.next(tile, k_begin, k_end);  // entry idx + 1
@@ -813,14 +891,16 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1) gemm_tc_kernel(cons
       gemm_stage_half<0>(acc_half, acc0, wl, lane);
       gemm_stage_half<0>(acc_half + 64 * kAccCols, acc1, wl, lane);
       bar_sync(3 + wg, 128);
-      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN, kAccCols, m_tile, r, []() {},
-                                                       stage_buf, store_groups, tr, kb == 0, seg);
+      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES, RAGGED>(p, acc_row, n_tile * kGemmBN, kAccCols, m_tile, r, []() {},
+                                                               stage_buf, store_groups, tr, kb == 0, seg,
+                                                               gemm_ragged_k(p, img), gemm_ragged_koff(p, img));
       bar_sync(3 + wg, 128);
       gemm_stage_half<1>(acc_half, acc0, wl, lane);
       gemm_stage_half<1>(acc_half + 64 * kAccCols, acc1, wl, lane);
       bar_sync(3 + wg, 128);
-      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES>(p, acc_row, n_tile * kGemmBN + kAccCols, kAccCols, m_tile, r,
-                                                       []() {}, stage_buf, store_groups, tr, kb == 0, seg);
+      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES, RAGGED>(p, acc_row, n_tile * kGemmBN + kAccCols, kAccCols, m_tile,
+                                                               r, []() {}, stage_buf, store_groups, tr, kb == 0, seg,
+                                                               gemm_ragged_k(p, img), gemm_ragged_koff(p, img));
       tr(7);
     }
     if (EPI != EPI_DIRECT && elect_one_sync()) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem

@@ -49,7 +49,7 @@ static int g_mhsa_variant = 0;   // kernel the engine's ViT attention runs (lseg
 static int g_gemm_cluster_mode = 2;  // lseg_debug_set_gemm_cluster: 1 never, 2 the planner's rule, 3 wherever allowed
 // Which gemm_tc_kernel instantiation runs a plan (numbering of lseg_debug_gemm_plan's out[4]).
 enum GemmKernel { GK_DIRECT = 0, GK_TMA_F16 = 1, GK_TMA_ADD = 2, GK_FIXED_SPLIT = 3, GK_GROUPED_NCHW = 4, GK_RELU_RES = 5,
-                  GK_COUNT = 6 };
+                  GK_RAGGED = 6, GK_COUNT = 7 };
 static int g_gemm_active_pairs[GK_COUNT];  // per instantiation: 2-CTA clusters of it that fit on the device at once
 static std::mutex g_init_mutex;
 static bool g_global_init = false;
@@ -122,10 +122,13 @@ static int init_device(int dev) {
       gemm_init_kernel<EPI_TMA_ADD>(&pairs[GK_TMA_ADD]) ||
       gemm_init_kernel<EPI_DIRECT, true>(&pairs[GK_FIXED_SPLIT]) ||
       gemm_init_kernel<EPI_DIRECT, false, true>(&pairs[GK_GROUPED_NCHW]) ||
-      gemm_init_kernel<EPI_DIRECT, false, false, true>(&pairs[GK_RELU_RES])) {
+      gemm_init_kernel<EPI_DIRECT, false, false, true>(&pairs[GK_RELU_RES]) ||
+      cudaFuncSetAttribute(gemm_tc_kernel<EPI_DIRECT, false, false, false, false, true>,
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<EPI_DIRECT>::kSmemBytes) != cudaSuccess) {
     set_error("lseg_b200: GEMM kernel attributes / cluster occupancy query failed on device %d", dev);
     return -1;
   }
+  pairs[GK_RAGGED] = 0;  // the ragged kernel has no clustered form
   memcpy(g_gemm_active_pairs, pairs, sizeof(pairs));
   cudaFuncSetAttribute(mhsa_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   cudaFuncSetAttribute(mhsa_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
@@ -223,6 +226,8 @@ struct GemmPlan {
   // workspace the CALLER provides (gemm_set_workspace) before gemm_run; final_epi is the epilogue the reduce applies
   size_t ws_bytes;
   GemmEpi final_epi;
+  int ragged = 0;      // 1: pixel x text over the per-image problem table rt (gemm_plan_ragged); never clustered
+  GemmRaggedTable rt;
 };
 
 // Split the K loop of the implicit-GEMM convs whose tile count leaves most CTAs idle (3x3 convs on the 15x15 decoder
@@ -267,8 +272,9 @@ static int gemm_kernel_of(const GemmPlan& plan);
 static int gemm_plan_grid(const GemmDesc& d, GemmPlan* plan) {
   GemmParams& p = plan->p;
   const int pairs = g_gemm_active_pairs[gemm_kernel_of(*plan)];
-  const int units = p.num_m_tiles * p.num_n_tiles * (p.split_fixed > 1 ? p.split_fixed : 1);
-  const bool allowed = p.num_n_tiles % 2 == 0 && !p.split_k && pairs > 0;
+  const int units = plan->ragged ? plan->rt.tile0[plan->rt.n]
+                                 : p.num_m_tiles * p.num_n_tiles * (p.split_fixed > 1 ? p.split_fixed : 1);
+  const bool allowed = !plan->ragged && p.num_n_tiles % 2 == 0 && !p.split_k && pairs > 0;
   const bool wanted = g_gemm_cluster_mode == 3 || (g_gemm_cluster_mode == 2 && units > g_num_sms);
   plan->cluster = (allowed && wanted) ? 2 : 1;
   if (plan->cluster == 2)
@@ -412,6 +418,44 @@ static int gemm_plan(const GemmDesc& d, GemmPlan* plan) {
   return gemm_plan_grid(d, plan);
 }
 
+// Ragged pixel x text plan (gemm_tc_kernel RAGGED, the table in gemm_tc.cuh): d describes the whole product — A = the
+// B * P pixel rows (P = d.e.nchw_p, a multiple of 128), w = the packed text operand with d.w_rows readable rows, e = the
+// NCHW-T epilogue whose out_f16 is the packed fp16 [sum k, P] output. Image b's label count k[b] and first text row
+// text_row[b] are host arrays: the tile counts are needed here. Unclustered: the pair rule needs an even n-tile count,
+// and the per-image counts are generally odd.
+static int gemm_plan_ragged(GemmDesc d, int B, const int* k, const int* text_row, GemmPlan* plan) {
+  const int P = d.e.nchw_p;
+  if (B < 1 || B > kRaggedMaxImages) return set_error("gemm_ragged: B=%d images (1 .. %d)", B, kRaggedMaxImages), -1;
+  if (P <= 0 || P % kGemmBM != 0 || static_cast<long long>(B) * P != d.M)
+    return set_error("gemm_ragged: P=%d pixels per image must be a positive multiple of %d (M=%d)", P, kGemmBM, d.M), -1;
+  GemmRaggedTable& rt = plan->rt;
+  memset(&rt, 0, sizeof(rt));
+  rt.n = B;
+  rt.m_tiles = P / kGemmBM;
+  long long koff = 0, tiles = 0;
+  int kmax = 0;
+  for (int b = 0; b < B; ++b) {
+    if (k[b] < 1 || text_row[b] < 0 || static_cast<long long>(text_row[b]) + k[b] > d.w_rows)
+      return set_error("gemm_ragged: image %d: k=%d labels at text_row=%d do not fit %d text rows", b, k[b], text_row[b],
+                       d.w_rows), -1;
+    rt.k[b] = k[b];
+    rt.text_row[b] = text_row[b];
+    rt.koff[b] = static_cast<int>(koff);
+    rt.tile0[b] = static_cast<int>(tiles);
+    koff += k[b];
+    tiles += static_cast<long long>(rt.m_tiles) * ((k[b] + kGemmBN - 1) / kGemmBN);
+    if (koff > 65535 || tiles > (1 << 30)) return set_error("gemm_ragged: sum of k = %lld exceeds 65535", koff), -1;
+    kmax = k[b] > kmax ? k[b] : kmax;
+  }
+  rt.tile0[B] = static_cast<int>(tiles);
+  d.N = kmax;
+  d.e.store = STORE_NCHW_T;
+  d.e.nchw_k = kmax;
+  d.e.nchw_group = 0;
+  plan->ragged = 1;
+  return gemm_plan(d, plan);
+}
+
 static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream);
 static int gemm_run(const GemmPlan& plan, cudaStream_t stream) {
   if (plan.grid <= 0) return 0;
@@ -431,6 +475,7 @@ static int gemm_run(const GemmPlan& plan, cudaStream_t stream) {
   return gemm_run_kernel(plan, stream);
 }
 static int gemm_kernel_of(const GemmPlan& plan) {
+  if (plan.ragged) return GK_RAGGED;
   if (plan.epi == EPI_TMA_F16) return GK_TMA_F16;
   if (plan.epi == EPI_TMA_ADD) return GK_TMA_ADD;
   if (plan.p.split_fixed > 1) return GK_FIXED_SPLIT;
@@ -454,6 +499,14 @@ static int gemm_run_kernel(const GemmPlan& plan, cudaStream_t stream) {
     case GK_FIXED_SPLIT: gemm_launch<EPI_DIRECT, true>(plan, stream); break;
     case GK_GROUPED_NCHW: gemm_launch<EPI_DIRECT, false, true>(plan, stream); break;
     case GK_RELU_RES: gemm_launch<EPI_DIRECT, false, false, true>(plan, stream); break;
+    case GK_RAGGED: {
+      GemmRaggedParams rp;
+      static_cast<GemmParams&>(rp) = plan.p;
+      rp.rt = plan.rt;
+      launch_pdl(gemm_tc_kernel<EPI_DIRECT, false, false, false, false, true>, dim3(plan.grid),
+                 dim3(GemmCfg<EPI_DIRECT>::kThreads), GemmCfg<EPI_DIRECT>::kSmemBytes, stream, rp);
+      break;
+    }
     default: gemm_launch<EPI_DIRECT>(plan, stream); break;
   }
   LSEG_CHECK_CUDA(cudaGetLastError());
@@ -652,6 +705,40 @@ int lseg_gemm(const lseg_gemm_args* a, void* stream) {
     }
     gemm_set_workspace(&plan, scratch[dev]);
   }
+  return gemm_run(plan, static_cast<cudaStream_t>(stream));
+}
+
+int lseg_gemm_ragged(const void* a, const float* row_sumsq, int row_sumsq_parts, float row_scale, int B, int P, int C,
+                     const void* text, int text_rows, const int* text_row, const int* k, void* out, void* stream) {
+  const char* fn = "lseg_gemm_ragged";
+  if (!a) return set_error("%s: null a", fn), -1;
+  if (!out) return set_error("%s: null out", fn), -1;
+  if (reinterpret_cast<uintptr_t>(a) % 16) return set_error("%s: a must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(out) % 16) return set_error("%s: out must be 16-byte aligned", fn), -1;
+  if (P <= 0 || P % kGemmBM != 0) return set_error("%s: P=%d must be a positive multiple of %d", fn, P, kGemmBM), -1;
+  if (C <= 0 || C % kGemmBK != 0) return set_error("%s: C=%d must be a positive multiple of %d", fn, C, kGemmBK), -1;
+  if (row_sumsq && row_sumsq_parts < 1)
+    return set_error("%s: row_sumsq_parts=%d must be positive with row_sumsq", fn, row_sumsq_parts), -1;
+  long long sum_k = 0;
+  if (check_ragged(fn, B, text, text_rows, text_row, k, &sum_k)) return -1;
+  if (static_cast<long long>(B) * P > (1ll << 31) - 1) return set_error("%s: B*P = %lld rows", fn, (long long)B * P), -1;
+  GemmDesc d;
+  memset(&d, 0, sizeof(d));
+  d.a = static_cast<const __half*>(a);
+  d.lda = C;
+  d.a_rows = B * P;
+  d.w = static_cast<const __half*>(text);
+  d.w_rows = text_rows;
+  d.M = B * P;
+  d.K = C;
+  d.e = epi_none();
+  d.e.out_f16 = static_cast<__half*>(out);
+  d.e.nchw_p = P;
+  d.e.row_sumsq = row_sumsq;
+  d.e.row_sumsq_parts = row_sumsq ? row_sumsq_parts : 0;
+  d.e.row_scale = row_scale;
+  GemmPlan plan;
+  if (gemm_plan_ragged(d, B, k, text_row, &plan)) return -1;
   return gemm_run(plan, static_cast<cudaStream_t>(stream));
 }
 

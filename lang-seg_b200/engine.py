@@ -231,6 +231,44 @@ class Engine:
                                            C.c_void_p(text.data_ptr()), k, text_image_stride, lp, mp, tp, gp,
                                            nclass, stats.shape[0] if stats is not None else 0, sp, _stream()))
 
+    def _ragged_args(self, text, text_row, k, b, h, w, logits, mask):
+        """ctypes arguments of a ragged call (include/lseg_b200.h), after checking the output tensors' shapes."""
+        if len(text_row) != b or len(k) != b:
+            raise ValueError(f"text_row and k need one entry per image ({b}), got {len(text_row)} and {len(k)}")
+        if text.device != self.device or text.dtype != torch.float16 or text.dim() != 2 or not text.is_contiguous():
+            raise ValueError(f"text must be a contiguous float16 [rows, out_c] tensor on {self.device}")
+        if logits is None and mask is None:
+            raise ValueError("ragged call: no output requested (logits or mask)")
+        for name, t, dt, shape in (("mask", mask, torch.int64, (b, h, w)), ("logits", logits, torch.float32,
+                                                                            (sum(k), h, w))):
+            if t is not None and (t.device != self.device or t.dtype != dt or tuple(t.shape) != shape or
+                                  not t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous {dt} {shape} tensor on {self.device}")
+        ints = C.c_int * b
+        return [C.c_void_p(text.data_ptr()), text.shape[0], ints(*text_row), ints(*k),
+                C.c_void_p(logits.data_ptr()) if logits is not None else None,
+                C.c_void_p(mask.data_ptr()) if mask is not None else None, _stream()]
+
+    def forward_ragged(self, x, text, text_row, k, logits=None, mask=None):
+        """Forward of a batch in which image b has its own k[b] labels, rows text_row[b] .. of `text` (fp16 [rows,
+        out_c]). Writes the packed fp32 logits [sum k, H, W] (image b's planes follow those of images 0 .. b-1) and / or
+        the int64 mask [B, H, W] (mask[b] indexes image b's labels) into the tensors passed. Enqueues on the current
+        stream."""
+        self._check_input(x)
+        x = x.contiguous()
+        b, _, h, w = x.shape
+        args = self._ragged_args(text, text_row, k, b, h, w, logits, mask)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_forward_ragged(self.handle, C.c_void_p(x.data_ptr()), b, h, w, *args))
+
+    def query_ragged(self, emb, sumsq, text, text_row, k, logits=None, mask=None):
+        """forward_ragged's label-dependent tail on a stored embedding pair."""
+        b, h, w = check_embedding(emb, sumsq, self.device, self.out_c)
+        args = self._ragged_args(text, text_row, k, b, h, w, logits, mask)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_query_ragged(self.handle, C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()),
+                                                  b, h, w, *args))
+
     def forward_profiled(self, x, text, k, text_image_stride=0, out=None):
         """One forward with CUDA events around every launch. Returns (out, [(ms, kind, flops), ...])."""
         x = x.contiguous()

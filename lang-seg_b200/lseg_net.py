@@ -180,6 +180,31 @@ _IGNORED_PREFIXES = ("clip_pretrained.visual.", "pretrained.model.head.", "pretr
 _WEIGHTS_GENERATION = itertools.count(1)  # process-wide: an embedding of another net never matches either
 
 
+def is_ragged(labelset):
+    """True for a per-image list of label lists (list[list[str]]): every image of the batch has its own label set."""
+    return isinstance(labelset, (list, tuple)) and any(isinstance(l, (list, tuple)) for l in labelset)
+
+
+def ragged_label_table(labelsets):
+    """Host tables of a batch in which image b has its own labels labelsets[b] -> (union, rows, k, koff):
+      union  the distinct labels of the batch in first-appearance order: each is tokenized and encoded once
+      rows   the union index of every row of the packed text operand; image b's labels are rows koff[b] .. koff[b]+k[b]-1
+      k      label count of every image
+      koff   first packed text row of every image, which is also its first plane of the packed logits (prefix sum of k)"""
+    index, union, rows, k, koff = {}, [], [], [], []
+    for b, labels in enumerate(labelsets):
+        if not isinstance(labels, (list, tuple)) or not labels or not all(isinstance(n, str) for n in labels):
+            raise ValueError(f"labelsets[{b}] must be a non-empty list of label strings, got {labels!r}")
+        koff.append(len(rows))
+        k.append(len(labels))
+        for name in labels:
+            if name not in index:
+                index[name] = len(union)
+                union.append(name)
+            rows.append(index[name])
+    return union, rows, k, koff
+
+
 class PixelEmbedding:
     """LSeg's pixel embedding of B images, as `LSegNet.encode_image` returns it: the output of the image path (trunk,
     decoder, head1; lseg_net.py:166-185) that every label set is then queried against. Pass it wherever the net takes
@@ -396,6 +421,33 @@ class _LSegBase(nn.Module):
         emb, sumsq = engine.encode_image(x.float())
         return PixelEmbedding(emb, sumsq, x.shape[2:], self.backbone, self.out_c, self._shared["generation"])
 
+    def _ragged_text(self, engine, labelsets, b):
+        """Packed text operand of a ragged batch: the union of its labels encoded once (through the text-feature cache),
+        then one device gather into image order, rows padded to a multiple of 128. -> (text, k, koff)."""
+        if len(labelsets) != b:
+            raise ValueError(f"{len(labelsets)} label sets for a batch of {b} images: one list of labels per image")
+        union, rows, k, koff = ragged_label_table(labelsets)
+        feats = self._text_features(engine, tokenize(union))
+        text = torch.zeros((engine.padded_rows(len(rows)), self.out_c), dtype=torch.float16, device=engine.device)
+        text[: len(rows)] = feats.index_select(0, torch.tensor(rows, dtype=torch.int64).to(engine.device))
+        return text, k, koff
+
+    def _run_ragged(self, x, labelsets, want_logits):
+        """Forward (want_logits) or predict of a batch whose image b has its own labels labelsets[b]."""
+        emb = x if isinstance(x, PixelEmbedding) else None
+        engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
+        b, h, w = x.shape[0], x.shape[2], x.shape[3]
+        text, k, koff = self._ragged_text(engine, labelsets, b)
+        logits = torch.empty((sum(k), h, w), dtype=torch.float32, device=x.device) if want_logits else None
+        mask = None if want_logits else torch.empty((b, h, w), dtype=torch.int64, device=x.device)
+        if emb is not None:
+            engine.query_ragged(emb.emb, emb.sumsq, text, koff, k, logits=logits, mask=mask)
+        else:
+            engine.forward_ragged(x.float(), text, koff, k, logits=logits, mask=mask)
+        if not want_logits:
+            return mask
+        return [logits[o:o + n].unsqueeze(0) for o, n in zip(koff, k)]
+
     def _embedding_engine(self, emb):
         """The engine that queries `emb`, after checking that this net's current weights produced it."""
         if emb.backbone != self.backbone or emb.out_c != self.out_c:
@@ -435,8 +487,14 @@ class LSegNet(_LSegBase):
 
     @torch.no_grad()
     def forward(self, x, labelset="", out=None):
-        """`out` (optional, beyond the reference signature): a contiguous fp32 [B,K,H,W] CUDA tensor to write into."""
+        """`out` (optional, beyond the reference signature): a contiguous fp32 [B,K,H,W] CUDA tensor to write into.
+        `labelset` may also be a list of B label lists, one per image: the result is then a list of B fp32 tensors
+        [1, k_b, H, W] (views of one packed buffer), each what forward(x[b:b+1], labelset[b]) returns."""
         self._check_eval()
+        if is_ragged(labelset):
+            if out is not None:
+                raise ValueError("out= is not supported with per-image label sets: the result is one tensor per image")
+            return self._run_ragged(x, labelset, want_logits=True)
         if isinstance(labelset, torch.Tensor):
             text = labelset
         elif isinstance(labelset, str) and labelset == "":
@@ -469,8 +527,10 @@ class LSegNet(_LSegBase):
     def predict(self, x, labelset=""):
         """torch.max(self.forward(x, labelset), 1)[1] — what every caller of the reference does with the logits
         (lseg_app.py:357-360, test_lseg.py:397) — fused on the device: int64 [B,H,W], the fp32 [B,K,H,W] logits are
-        never written (SURVEY.md 8(f) row 2)."""
+        never written (SURVEY.md 8(f) row 2). With a list of B label lists, mask[b] indexes labelset[b]."""
         self._check_eval()
+        if is_ragged(labelset):
+            return self._run_ragged(x, labelset, want_logits=False)
         text = self._labelset_tokens(labelset)
         if isinstance(x, PixelEmbedding):
             engine = self._embedding_engine(x)
@@ -488,6 +548,9 @@ class LSegNet(_LSegBase):
         ignored) are added on the device. Neither logits nor mask are written, and nothing synchronises."""
         from .metrics import _as_target
         self._check_eval()
+        if is_ragged(labelset):
+            raise ValueError("update_metric does not take per-image label sets: the class ids of the metric would differ "
+                             "from image to image")
         text = self._labelset_tokens(labelset)
         emb = x if isinstance(x, PixelEmbedding) else None
         engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)

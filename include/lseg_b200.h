@@ -118,6 +118,15 @@ int lseg_mhsa(const void* qkv, void* out, int B, int N, int heads, int causal, v
  * evaluated on the FMA pipe instead of the MUFU pipe: 0, 1, 2, 5, 6 = none; 3, 7 = one of every four score pairs;
  * 4, 8 = two of four. */
 int lseg_mhsa_variant(const void* qkv, void* out, int B, int N, int heads, int causal, int variant, void* stream);
+/* Attention probabilities, head_dim 64, non-causal: the tensor the reference's attention hook records (get_attention,
+ * lseg_vit.py:22-42). qkv fp16 [B, N, 3*heads*64] (q|k|v thirds, as lseg_mhsa reads it) -> out fp32 [B, heads, N, N],
+ * contiguous: out[b, h, i, j] = softmax_j(0.125 * q_i . k_j) of head h, with q, k the fp16 rows, the scores accumulated
+ * in fp32 by the tensor cores and normalised with the row's final max and sum (two passes over the keys). Only the
+ * B*heads*N*N elements are written. Same rules as lseg_mhsa: B, N and heads positive with B*heads <= 65535; qkv 16-byte
+ * aligned (TMA loads); out 4-byte aligned (the row pitch 4N is generally not a multiple of 16, so the kernel stores
+ * single floats). A call that breaks one of them is rejected with an error naming the argument, before anything is
+ * launched. Enqueued on `stream`. */
+int lseg_attn_probs(const void* qkv, float* out, int B, int N, int heads, void* stream);
 /* Causal attention of the CLIP text tower with the rounding points of torch's multi_head_attention_forward on fp16
  * tensors (q*dh^-0.5, bmm -> fp16, softmax -> fp16 normalised, bmm -> fp16; SURVEY.md Appendix A.2): CUDA cores, one
  * CTA per (label, head). qkv fp16 [K, L, 3*heads*64] -> out fp16 [K*L, heads*64]. 1 <= L <= 80, 1 <= K <= 65535 and
@@ -428,6 +437,17 @@ int lseg_forward_profiled(lseg_engine* e, const float* x, int B, int H, int W, c
  * image path; head1 stores straight into the caller's buffers. */
 int lseg_encode_image(lseg_engine* e, const float* x, int B, int H, int W,
                       void* emb /* fp16 [B,H/2,W/2,out_c] */, float* emb_sumsq /* fp32 [B,H/2,W/2,out_c/32] */, void* stream);
+
+/* lseg_encode_image that also records the ViT's attention maps (the reference's enable_attention_hooks, lseg_vit.py:428-441:
+ * pretrained.attention["attn_1".."attn_4"]). Same launches and output bits as lseg_encode_image, plus one launch per
+ * hooked block: attn[k] receives fp32 [B, heads, N, N] (N = (H/patch)*(W/patch) + 1 tokens, contiguous) = the softmax
+ * probabilities of block hooks[k] (lseg_attn_probs on that block's QKV rows, run right after the block's attention, while
+ * the rows are still in the workspace). The four buffers belong to the caller (no workspace grows); each must be non-NULL
+ * and 4-byte aligned, and the engine must have a ViT trunk (not the ResNet-101 one). Every rule is checked, and rejected
+ * by name, before the first launch. Plans that record attention are cached apart from those that do not, so a forward
+ * without it runs exactly the launches it ran before. */
+int lseg_encode_image_attention(lseg_engine* e, const float* x, int B, int H, int W, void* emb, float* emb_sumsq,
+                                float* const attn[4], void* stream);
 
 /* The label-dependent tail of LSeg.forward on an embedding of B images of H x W. text / K / text_image_stride as in
  * lseg_forward. Outputs, each nullable, at least one requested; each equals what the corresponding forward entry point

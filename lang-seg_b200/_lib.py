@@ -99,6 +99,7 @@ SYMBOLS = [
     "lseg_seg_stats_scores", "lseg_seg_stats_mask", "lseg_forward_segstats",
     "lseg_encode_image", "lseg_query", "lseg_embedding_features",
     "lseg_forward_ragged", "lseg_query_ragged", "lseg_gemm_ragged",
+    "lseg_attn_probs", "lseg_encode_image_attention",
 ]
 
 _lib = None
@@ -136,6 +137,7 @@ def load(build_if_missing=True):
     lib.lseg_debug_set_gemm_cluster.argtypes = [C.c_int]
     lib.lseg_mhsa.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_mhsa_variant.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib.lseg_attn_probs.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_text_attn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_debug_gemm_trace.argtypes = [C.c_void_p]
     lib.lseg_set_deterministic.argtypes = [C.c_int]
@@ -200,6 +202,8 @@ def load(build_if_missing=True):
                                           C.c_void_p, C.c_void_p]
     lib.lseg_encode_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p]
+    lib.lseg_encode_image_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                                C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]
     lib.lseg_query.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                C.c_void_p, C.c_void_p]

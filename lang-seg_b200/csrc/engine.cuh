@@ -32,6 +32,9 @@ struct CallCtx {
   const int* rag_k = nullptr;
   const int* rag_text_row = nullptr;
   int rag_text_rows = 0;
+  // lseg_encode_image_attention: attn[k] receives the attention probabilities of block hooks[k], fp32 [B, heads, N, N]
+  // (read only by the steps of a plan built with ImagePlan::attn)
+  float* const* attn = nullptr;
 };
 using StepFn = std::function<int(const CallCtx&, cudaStream_t)>;
 enum StepKind { KIND_EW = 0, KIND_GEMM = 1, KIND_MHSA = 2, KIND_LN = 3, KIND_MEMSET = 4 };
@@ -87,6 +90,7 @@ struct Arena {
 struct ImagePlan {
   int B = 0, H = 0, W = 0;
   int epoch = 0;  // g_plan_epoch at build time (options baked into the GEMM plans)
+  bool attn = false;  // records the hooked blocks' attention probabilities into CallCtx::attn (one step per hooked block)
   Arena arena;
   std::vector<Step> steps;  // the trunk up to (not including) head1
   std::map<std::string, const void*> debug;
@@ -360,6 +364,18 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       steps.emplace_back([mp](const CallCtx&, cudaStream_t s) { return mhsa_run(mp, s); }, KIND_MHSA,
                          4.0 * B * heads * static_cast<double>(N) * N * 64);
     }
+    for (int k = 0; k < 4 && plan->attn; ++k) {  // the hook reads this block's q, k (lseg_vit.py:22-42): qkv holds them
+      if (w.hooks[k] != i) continue;             // until the next block's QKV GEMM overwrites it
+      AttnProbsPlan ap;
+      if (attn_probs_maps(qkv, B, N, heads, &ap)) return -1;
+      steps.emplace_back(
+          [ap, k](const CallCtx& c, cudaStream_t s) {
+            AttnProbsPlan run = ap;
+            run.p.out = c.attn[k];
+            return attn_probs_run(run, s);
+          },
+          KIND_MHSA, 4.0 * B * heads * static_cast<double>(N) * N * 64);
+    }
     {
       GemmEpi e = epi_none();
       e.bias = bw.proj.b;
@@ -615,13 +631,14 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
   return 0;
 }
 
-static int build_image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t stream) {
+static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cudaStream_t stream) {
   const lseg_weights& w = eng->w;
   std::unique_ptr<ImagePlan> plan(new ImagePlan());
   plan->B = B;
   plan->H = H;
   plan->W = W;
   plan->epoch = g_plan_epoch;
+  plan->attn = attn;
   Arena& arena = plan->arena;
   t_plan_arena = &arena;
   std::vector<Step>& steps = plan->steps;
@@ -802,8 +819,9 @@ static int check_image_shape(const char* fn, int B, int H, int W) {
   return 0;
 }
 
-// The image plan for (B, H, W), built on first use; plans built under other baked-in options are dropped.
-static ImagePlan* image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t stream) {
+// The image plan for (B, H, W), with or without the attention-recording steps, built on first use; plans built under
+// other baked-in options are dropped.
+static ImagePlan* image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t stream, bool attn = false) {
   eng->img = nullptr;
   for (size_t i = 0; i < eng->plans.size();) {
     ImagePlan* pl = eng->plans[i].get();
@@ -812,10 +830,10 @@ static ImagePlan* image_plan(lseg_engine* eng, int B, int H, int W, cudaStream_t
       eng->plans.erase(eng->plans.begin() + i);
       continue;
     }
-    if (pl->B == B && pl->H == H && pl->W == W) eng->img = pl;
+    if (pl->B == B && pl->H == H && pl->W == W && pl->attn == attn) eng->img = pl;
     ++i;
   }
-  if (!eng->img && build_image_plan(eng, B, H, W, stream)) return nullptr;
+  if (!eng->img && build_image_plan(eng, B, H, W, attn, stream)) return nullptr;
   eng->img->last_use = ++eng->use_counter;
   return eng->img;
 }
@@ -1468,6 +1486,42 @@ int lseg_encode_image(lseg_engine* e, const float* x, int B, int H, int W, void*
   CallCtx ctx;
   memset(&ctx, 0, sizeof(ctx));
   ctx.x = x;
+  int launches = 0;
+  if (run_trunk(e, *plan, ctx, static_cast<__half*>(emb), emb_sumsq, s, nullptr, &launches)) return -1;
+  e->last_launches = launches;
+  return 0;
+}
+
+int lseg_encode_image_attention(lseg_engine* e, const float* x, int B, int H, int W, void* emb, float* emb_sumsq,
+                                float* const attn[4], void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_encode_image_attention";
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!x) return set_error("%s: null x", fn), -1;
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 16) return set_error("%s: emb_sumsq must be 16-byte aligned", fn), -1;
+  if (!attn) return set_error("%s: null attn", fn), -1;
+  for (int k = 0; k < 4; ++k) {
+    if (!attn[k]) return set_error("%s: null attn[%d]", fn, k), -1;
+    if (reinterpret_cast<uintptr_t>(attn[k]) % 4) return set_error("%s: attn[%d] must be 4-byte aligned", fn, k), -1;
+  }
+  if (e->w.trunk != 0)
+    return set_error("%s: the engine has no ViT trunk (ResNet-101 weights): there are no attention maps", fn), -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  if (static_cast<long long>(B) * e->w.vit_heads > 65535)
+    return set_error("%s: B*heads = %lld exceeds 65535", fn, static_cast<long long>(B) * e->w.vit_heads), -1;
+  if (ensure_init()) return -1;
+  LSEG_CHECK_CUDA(cudaSetDevice(e->device));
+  if (ensure_init()) return -1;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  ImagePlan* plan = image_plan(e, B, H, W, s, true);
+  if (!plan) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.x = x;
+  ctx.attn = attn;
   int launches = 0;
   if (run_trunk(e, *plan, ctx, static_cast<__half*>(emb), emb_sumsq, s, nullptr, &launches)) return -1;
   e->last_launches = launches;

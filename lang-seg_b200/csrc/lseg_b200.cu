@@ -14,6 +14,7 @@
 #include "elementwise.cuh"
 #include "gemm_tc.cuh"
 #include "mhsa.cuh"
+#include "attn_probs.cuh"
 #include "text_attn.cuh"
 #include "p2p.cuh"
 #include "evaluator.cuh"
@@ -134,6 +135,7 @@ static int init_device(int dev) {
   cudaFuncSetAttribute(mhsa_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   cudaFuncSetAttribute(mhsa_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
   cudaFuncSetAttribute(mhsa_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMhsaSmemBytes);
+  cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnPSmemBytes);
   if (cudaGetLastError() != cudaSuccess) {
     set_error("lseg_b200: cudaFuncSetAttribute failed on device %d", dev);
     return -1;
@@ -581,6 +583,57 @@ static int mhsa_run_variant(const MhsaPlan& plan, int variant, cudaStream_t stre
 static int mhsa_run(const MhsaPlan& plan, cudaStream_t stream) { return mhsa_run_variant(plan, g_mhsa_variant, stream); }
 
 // ------------------------------------------------------------------------------------------
+// attention probabilities (attn_probs.cuh): planning / launch
+// ------------------------------------------------------------------------------------------
+struct AttnProbsPlan {
+  AttnProbsParams p;  // p.out is set per call (the engine's plans take it from CallCtx)
+  dim3 grid;
+};
+// Tensor maps and grid for qkv of (B, N, heads), whose arguments have been checked: those of the fused attention kernel.
+static int attn_probs_maps(const __half* qkv, int B, int N, int heads, AttnProbsPlan* plan) {
+  MhsaDesc d;
+  d.qkv = qkv;
+  d.out = const_cast<__half*>(qkv);  // mhsa_plan wants an output; this one is never written
+  d.B = B;
+  d.N = N;
+  d.heads = heads;
+  d.causal = 0;
+  MhsaPlan mp;
+  if (mhsa_plan(d, &mp)) return -1;
+  AttnProbsParams& p = plan->p;
+  memset(&p, 0, sizeof(p));
+  p.tma_qkv = mp.p.tma_qkv;
+  p.tma_t64 = mp.p.tma_t64;
+  p.n_tokens = N;
+  p.heads = heads;
+  p.D = mp.p.D;
+  p.scale_log2e = mp.p.scale_log2e;
+  plan->grid = mp.grid;
+  return 0;
+}
+// The rules of lseg_attn_probs (include/lseg_b200.h), each rejected by name before a tensor map is encoded.
+static int attn_probs_plan(const char* fn, const __half* qkv, float* out, int B, int N, int heads, AttnProbsPlan* plan) {
+  if (B <= 0) return set_error("%s: B=%d must be positive", fn, B), -1;
+  if (N <= 0) return set_error("%s: N=%d must be positive", fn, N), -1;
+  if (heads <= 0) return set_error("%s: heads=%d must be positive", fn, heads), -1;
+  if (static_cast<long long>(B) * heads > 65535)
+    return set_error("%s: B*heads = %lld exceeds 65535 (B=%d, heads=%d)", fn, static_cast<long long>(B) * heads, B, heads),
+           -1;
+  if (!qkv) return set_error("%s: null qkv", fn), -1;
+  if (reinterpret_cast<uintptr_t>(qkv) % 16) return set_error("%s: qkv must be 16-byte aligned", fn), -1;
+  if (!out) return set_error("%s: null out", fn), -1;
+  if (reinterpret_cast<uintptr_t>(out) % 4) return set_error("%s: out must be 4-byte aligned", fn), -1;
+  if (attn_probs_maps(qkv, B, N, heads, plan)) return -1;
+  plan->p.out = out;
+  return 0;
+}
+static int attn_probs_run(const AttnProbsPlan& plan, cudaStream_t stream) {
+  launch_pdl(attn_probs_kernel, plan.grid, dim3(kAttnPThreads), kAttnPSmemBytes, stream, plan.p);
+  LSEG_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
 // elementwise launch helpers
 // ------------------------------------------------------------------------------------------
 static int run_layernorm(const void* x, int in_f16, const float* g, const float* b, __half* y, long long M, int C,
@@ -766,6 +819,12 @@ int lseg_mhsa_variant(const void* qkv, void* out, int B, int N, int heads, int c
   MhsaPlan plan;
   if (mhsa_plan(d, &plan)) return -1;
   return mhsa_run_variant(plan, variant, static_cast<cudaStream_t>(stream));
+}
+
+int lseg_attn_probs(const void* qkv, float* out, int B, int N, int heads, void* stream) {
+  AttnProbsPlan plan;
+  if (attn_probs_plan("lseg_attn_probs", static_cast<const __half*>(qkv), out, B, N, heads, &plan)) return -1;
+  return attn_probs_run(plan, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_text_attn(const void* qkv, void* out, int K, int L, int heads, void* stream) {

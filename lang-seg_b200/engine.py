@@ -198,6 +198,34 @@ class Engine:
                                                   C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()), _stream()))
         return emb, sumsq
 
+    def attention_shape(self, b, h, w):
+        """Shape of one hooked block's attention probabilities for B images of H x W: [B, heads, N, N] with N the
+        token count (patch grid + class token)."""
+        d = self.weights.desc
+        if d.trunk != 0:
+            raise ValueError("attention maps need a ViT trunk; this engine runs the ResNet-101 one")
+        p = int(d.patch_size)
+        n = (h // p) * (w // p) + 1
+        return (b, int(d.vit_heads), n, n)
+
+    def encode_image_attention(self, x):
+        """encode_image that also records the attention probabilities of the four hooked blocks: returns (emb, sumsq,
+        [attn_1, .., attn_4]), each attn_k a fresh fp32 [B, heads, N, N] tensor. The embedding pair has the same bits as
+        encode_image's. Enqueues on the current stream."""
+        self._check_input(x)
+        x = x.contiguous()
+        b, _, h, w = x.shape
+        shape = self.attention_shape(b, h, w)
+        emb = torch.empty((b, h // 2, w // 2, self.out_c), dtype=torch.float16, device=self.device)
+        sumsq = torch.empty((b, h // 2, w // 2, self.out_c // 32), dtype=torch.float32, device=self.device)
+        attn = [torch.empty(shape, dtype=torch.float32, device=self.device) for _ in range(4)]
+        ptrs = (C.c_void_p * 4)(*[a.data_ptr() for a in attn])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_encode_image_attention(self.handle, C.c_void_p(x.data_ptr()), b, h, w,
+                                                            C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()),
+                                                            ptrs, _stream()))
+        return emb, sumsq, attn
+
     def query(self, emb, sumsq, text, k, text_image_stride=0, logits=None, mask=None, target=None, stats=None,
               nclass=0, group=None):
         """The label-dependent tail of forward on a stored embedding: writes the fp32 logits [B,K,H,W] (as forward), the

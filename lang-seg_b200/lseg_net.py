@@ -7,6 +7,9 @@ Mirrors the reference interface for the hot path (SURVEY.md section 8(b)):
   * attributes the callers touch: `.pretrained.model.patch_embed.img_size` (lseg_module.py:86-89),
     `.scratch`, `.clip_pretrained` (with `.encode_text`), `.labels`, `.text`, `.crop_size`, `.out_c`,
     `.arch_option`, `.logit_scale`;
+  * `enable_attention_hooks=True` (the `_make_encoder` argument, lseg_blocks.py:22) on a ViT-L/16 backbone: every call
+    that runs the image path records the hooked blocks' attention probabilities in `.pretrained.attention`
+    (lseg_vit.py:428-441), and `get_mean_attention_map` (lseg_vit.py:45-54) turns one token's row into an image map;
   * state-dict key names and shapes of SURVEY.md Appendix C, so `BaseModel.load` / Lightning's
     `load_from_checkpoint` (prefix `net.`) keep working; the unused `clip_pretrained.visual.*` and timm
     `head.*` entries of real checkpoints are accepted and ignored.
@@ -180,6 +183,23 @@ _IGNORED_PREFIXES = ("clip_pretrained.visual.", "pretrained.model.head.", "pretr
 _WEIGHTS_GENERATION = itertools.count(1)  # process-wide: an embedding of another net never matches either
 
 
+def get_mean_attention_map(attn, token, shape):
+    """modules/models/lseg_vit.py:45-54 in plain torch: the attention row of query `token` over the patch keys of attn
+    [B, heads, N, N] (as `.pretrained.attention["attn_k"]` holds it), unflattened to the token grid of an image of
+    shape[2:] (H, W), upsampled bicubically (align_corners=False) to H x W, then averaged over dim 0.
+
+    The reference's quirks are kept, so results match it call for call:
+      * the grid is shape[2] // 16 x shape[3] // 16 whatever the backbone's patch size (both ViT-L/16 backbones record);
+      * `.squeeze(0)` then `mean(0)`: for B = 1 the squeeze drops the batch and the mean runs over the heads -> [H, W];
+        for B > 1 nothing is squeezed and the mean runs over the IMAGES -> [heads, H, W].
+    Not on the hot path: no CUDA needed (CPU or CUDA tensors)."""
+    attn = attn[:, :, token, 1:]
+    attn = attn.unflatten(2, torch.Size([shape[2] // 16, shape[3] // 16])).float()
+    attn = torch.nn.functional.interpolate(attn, size=shape[2:], mode="bicubic", align_corners=False).squeeze(0)
+    all_attn = torch.mean(attn, 0)
+    return all_attn
+
+
 def is_ragged(labelset):
     """True for a per-image list of label lists (list[list[str]]): every image of the batch has its own label set."""
     return isinstance(labelset, (list, tuple)) and any(isinstance(l, (list, tuple)) for l in labelset)
@@ -293,6 +313,11 @@ class _LSegBase(nn.Module):
                 hb.depthwise.depthwise = nn.Conv2d(1, 1, kernel_size=3, stride=1, padding=1)
                 self.scratch.head_block = hb
         self.logit_scale = torch.tensor(reference_logit_scale())
+        # enable_attention_hooks (lseg_blocks.py:22): only the ViT-L/16 encoders honour it; _make_pretrained_clip_vitb32_384
+        # forces it off (lseg_vit.py:270) and the ResNet trunk has no attention
+        self._records_attention = bool(kwargs.get("enable_attention_hooks", False)) and cfg.get("patch") == 16
+        if self._records_attention:
+            self.pretrained.attention = {}  # per net (the reference's dict is module-global, lseg_vit.py:19)
         self.clip_pretrained._owner = weakref.ref(self)
         self._install_load_hooks()
         self._shared = {"engines": {}, "text_cache": {}, "lock": threading.Lock(), "master": weakref.ref(self),
@@ -415,11 +440,25 @@ class _LSegBase(nn.Module):
     @torch.no_grad()
     def encode_image(self, x):
         """The image path of forward (trunk, decoder, head1; lseg_net.py:166-185) of x fp32 [B,3,H,W] -> a
-        PixelEmbedding to pass to forward / predict / update_metric in place of x, with any label set."""
+        PixelEmbedding to pass to forward / predict / update_metric in place of x, with any label set. Records the
+        attention maps when the net was built with enable_attention_hooks."""
         self._check_eval()
         engine = self._engine_for(x.device)
-        emb, sumsq = engine.encode_image(x.float())
+        if self._records_attention:
+            emb, sumsq, attn = engine.encode_image_attention(x.float())
+            for k, a in enumerate(attn):  # fresh tensors: ones a caller kept from an earlier call stay as they were
+                self.pretrained.attention[f"attn_{k + 1}"] = a
+        else:
+            emb, sumsq = engine.encode_image(x.float())
         return PixelEmbedding(emb, sumsq, x.shape[2:], self.backbone, self.out_c, self._shared["generation"])
+
+    def _image_path(self, x):
+        """x as it goes to the engine: with enable_attention_hooks, images are encoded here (recording the attention
+        maps) and the call continues on the embedding, whose tail (lseg_query) is bit-identical to the fused forward; a
+        PixelEmbedding, or any input of a net that does not record, is returned as it is."""
+        if self._records_attention and not isinstance(x, PixelEmbedding):
+            return self.encode_image(x)
+        return x
 
     def _ragged_text(self, engine, labelsets, b):
         """Packed text operand of a ragged batch: the union of its labels encoded once (through the text-feature cache),
@@ -494,13 +533,18 @@ class LSegNet(_LSegBase):
         if is_ragged(labelset):
             if out is not None:
                 raise ValueError("out= is not supported with per-image label sets: the result is one tensor per image")
-            return self._run_ragged(x, labelset, want_logits=True)
+            return self._run_ragged(self._image_path(x), labelset, want_logits=True)
         if isinstance(labelset, torch.Tensor):
             text = labelset
         elif isinstance(labelset, str) and labelset == "":
             text = self.text
         else:
             text = tokenize(labelset)
+        if not isinstance(x, PixelEmbedding) and out is not None and (
+                out.dtype != torch.float32 or not out.is_contiguous() or
+                tuple(out.shape) != (x.shape[0], text.shape[0], x.shape[2], x.shape[3])):
+            raise ValueError("out must be a contiguous float32 [B,K,H,W] tensor")
+        x = self._image_path(x)
         if isinstance(x, PixelEmbedding):
             engine = self._embedding_engine(x)
             feats = self._text_features(engine, text)
@@ -511,9 +555,6 @@ class LSegNet(_LSegBase):
             return out
         engine = self._engine_for(x.device)
         feats = self._text_features(engine, text)
-        if out is not None and (out.dtype != torch.float32 or not out.is_contiguous() or
-                                tuple(out.shape) != (x.shape[0], text.shape[0], x.shape[2], x.shape[3])):
-            raise ValueError("out must be a contiguous float32 [B,K,H,W] tensor")
         return engine.forward(x.float(), feats, text.shape[0], out=out)
 
     def _labelset_tokens(self, labelset):
@@ -530,8 +571,9 @@ class LSegNet(_LSegBase):
         never written (SURVEY.md 8(f) row 2). With a list of B label lists, mask[b] indexes labelset[b]."""
         self._check_eval()
         if is_ragged(labelset):
-            return self._run_ragged(x, labelset, want_logits=False)
+            return self._run_ragged(self._image_path(x), labelset, want_logits=False)
         text = self._labelset_tokens(labelset)
+        x = self._image_path(x)
         if isinstance(x, PixelEmbedding):
             engine = self._embedding_engine(x)
             mask = torch.empty((len(x),) + x.size, dtype=torch.int64, device=x.device)
@@ -552,6 +594,7 @@ class LSegNet(_LSegBase):
             raise ValueError("update_metric does not take per-image label sets: the class ids of the metric would differ "
                              "from image to image")
         text = self._labelset_tokens(labelset)
+        x = self._image_path(x)
         emb = x if isinstance(x, PixelEmbedding) else None
         engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
         feats = self._text_features(engine, text)
@@ -605,6 +648,7 @@ class LSegNetZS(_LSegBase):
     @torch.no_grad()
     def forward(self, x, class_info):
         self._check_eval()
+        x = self._image_path(x)
         if isinstance(x, PixelEmbedding):
             engine = self._embedding_engine(x)
             out = torch.empty((len(x), 2) + x.size, dtype=torch.float32, device=x.device)
@@ -623,6 +667,7 @@ class LSegNetZS(_LSegBase):
     def predict(self, x, class_info):
         """argmax over the ['others', name] pair per pixel (test_lseg_zs.py:301), fused on the device."""
         self._check_eval()
+        x = self._image_path(x)
         if isinstance(x, PixelEmbedding):
             engine = self._embedding_engine(x)
             mask = torch.empty((len(x),) + x.size, dtype=torch.int64, device=x.device)
@@ -640,6 +685,7 @@ class LSegNetZS(_LSegBase):
         synchronisation is forward()'s class_info range check. A padded input takes a target padded with -1."""
         from .metrics import _as_target, _fewshot_target
         self._check_eval()
+        x = self._image_path(x)
         emb = x if isinstance(x, PixelEmbedding) else None
         engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
         text = self._image_text(engine, class_info, x.device)

@@ -138,6 +138,23 @@ def mhsa(qkv, B, N, heads, causal=False, variant=None, out=None):
     return out
 
 
+def attn_probs(qkv, heads, out=None):
+    """Attention probabilities softmax(0.125 * q k^T) of every head (include/lseg_b200.h lseg_attn_probs): qkv fp16
+    [B, N, 3*heads*64] -> fp32 [B, heads, N, N]. out: optional contiguous fp32 [B, heads, N, N] on qkv's device."""
+    if qkv.dim() != 3 or qkv.shape[2] != 3 * heads * 64:
+        raise _lib.LsegError(f"attn_probs: qkv must be [B, N, {3 * heads * 64}], got {list(qkv.shape)}")
+    B, N = qkv.shape[0], qkv.shape[1]
+    shape = (B, heads, N, N)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=qkv.device)
+    elif (out.dtype != torch.float32 or tuple(out.shape) != shape or out.device != qkv.device or
+          not out.is_contiguous()):
+        raise _lib.LsegError(f"attn_probs: out must be a contiguous fp32 {list(shape)} tensor on {qkv.device}, got "
+                             f"{out.dtype} {list(out.shape)} on {out.device}")
+    check(load().lseg_attn_probs(_ptr(qkv, torch.float16), _ptr(out), B, N, heads, _stream()))
+    return out
+
+
 def text_attn(qkv, K, L, heads, out=None):
     """Causal CLIP-text attention with torch's fp16 rounding points (include/lseg_b200.h lseg_text_attn).
     out: optional fp16 [K*L, heads*64]."""

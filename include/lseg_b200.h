@@ -149,6 +149,23 @@ int lseg_debug_gemm_trace(unsigned long long* trace);
 int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int causal, unsigned long long* trace,
                     void* stream);
 
+/* ---- glue entries (lseg_layernorm .. lseg_text_eot_gather, and lseg_preprocess) ----------------------------------------
+ * Each rejects, naming itself and the argument, before anything is launched and with its outputs untouched:
+ *   - a null pointer, or one not aligned to the kernel's vector width: 16 B for the float4 / uint4 operands (layernorm
+ *     x, gamma, beta, y; patchify x; assemble_tokens; readout_split tap; the NHWC kernels' x and y; the nchw upsamples'
+ *     x and y except the _bg source; l2norm_scale x), 8 B for uint2 stores and int64 tokens, else the element size;
+ *   - a size that is not positive;
+ *   - C % 8 != 0 for the uint4 NHWC kernels (im2col_3x3_s2, upsample2x_nhwc, maxpool, subsample), D % 4 != 0 for
+ *     assemble_tokens / readout_split;
+ *   - a shape the kernel is not built for: layernorm C not in {512, 768, 1024}; patch not in {16, 32} or not dividing
+ *     H and W; odd H or W for stem_im2col / maxpool / subsample; l2norm_scale C not a multiple of 128 or above 512;
+ *     W % 8 != 0 or W > 512 for upsample2x_nchw / _f32 / argmax, odd W for _bg; add with an fp16 nhwc256 output;
+ *     head_block mode not 1 / 2 or act not 0..3;
+ *   - a grid beyond its limit: 65535 in y / z (B of maxpool / subsample / the NHWC upsamples / im2col_3x3_s2, 2H of the
+ *     NHWC upsamples, B*H/P of patchify, ceil(h/8) and B*K of head_block, ceil(Hp/8) of preprocess, planes of the
+ *     nchw upsamples, B of upsample2x_argmax), 2^31 - 1 in x
+ *     (B*(H/2)*(W/2) of stem_im2col, 1 + gh*gw of pos_resize, the token rows of assemble / readout / text_embed). */
+
 /* LayerNorm over the last dim (k3): x fp32 (in_f16=0) or fp16 (in_f16=1) [M,C] -> y fp16. */
 int lseg_layernorm(const void* x, int in_f16, const float* gamma, const float* beta, void* y, long long M, int C,
                    float eps, void* stream);

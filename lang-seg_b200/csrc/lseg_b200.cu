@@ -661,6 +661,32 @@ static int run_layernorm(const void* x, int in_f16, const float* g, const float*
   return 0;
 }
 
+// Argument rules of the glue entries (include/lseg_b200.h): each is checked, and a violation reported by entry and
+// argument name, before anything is launched. Alignments are the kernels' vector widths; grid-y/z limits are 65535.
+constexpr long long kGridYZ = 65535, kGridX = 2147483647;
+static int arg_ptr(const char* fn, const char* name, const void* p, int align) {
+  if (!p) return set_error("%s: null %s", fn, name), -1;
+  if (reinterpret_cast<uintptr_t>(p) % align) return set_error("%s: %s must be %d-byte aligned", fn, name, align), -1;
+  return 0;
+}
+static int arg_pos(const char* fn, const char* name, long long v) {
+  if (v <= 0) return set_error("%s: %s=%lld must be positive", fn, name, v), -1;
+  return 0;
+}
+static int arg_max(const char* fn, const char* what, long long v, long long lim) {
+  if (v > lim) return set_error("%s: %s = %lld exceeds %lld", fn, what, v, lim), -1;
+  return 0;
+}
+static int arg_mult(const char* fn, const char* name, long long v, int m) {
+  if (v % m) return set_error("%s: %s=%lld must be a multiple of %d", fn, name, v, m), -1;
+  return 0;
+}
+// the smem-line upsamples (lseg_upsample2x_nchw*, lseg_upsample2x_argmax): W % 8 == 0, W <= kUpMaxW
+static int arg_up_w(const char* fn, int W) {
+  if (arg_mult(fn, "W", W, 8)) return -1;
+  return arg_max(fn, "W", W, kUpMaxW);
+}
+
 }  // namespace lseg
 
 #include "engine.cuh"
@@ -877,12 +903,15 @@ int lseg_eval_resize_add(const float* canvas, float* scores, int K, int height, 
 
 int lseg_preprocess(const unsigned char* img_hwc, float* out, int h, int w, int Ho, int Wo, int Hp, int Wp,
                     const float* mean3_host, const float* std3_host, const float* pad3_host, void* stream) {
-  if (ensure_init()) return -1;
-  if (!img_hwc || !out || !mean3_host || !std3_host || !pad3_host || h <= 0 || w <= 0 || Ho <= 0 || Wo <= 0 || Hp < Ho ||
-      Wp < Wo) {
-    set_error("lseg_preprocess: bad argument");
+  const char* fn = "lseg_preprocess";
+  if (arg_ptr(fn, "img_hwc", img_hwc, 1) || arg_ptr(fn, "out", out, 4) || arg_ptr(fn, "mean3", mean3_host, 4) ||
+      arg_ptr(fn, "std3", std3_host, 4) || arg_ptr(fn, "pad3", pad3_host, 4) || arg_pos(fn, "h", h) ||
+      arg_pos(fn, "w", w) || arg_pos(fn, "Ho", Ho) || arg_pos(fn, "Wo", Wo) ||
+      arg_max(fn, "ceil(Hp/8)", (static_cast<long long>(Hp) + 7) / 8, kGridYZ))
     return -1;
-  }
+  if (Hp < Ho) return set_error("%s: Hp=%d must be >= Ho=%d", fn, Hp, Ho), -1;
+  if (Wp < Wo) return set_error("%s: Wp=%d must be >= Wo=%d", fn, Wp, Wo), -1;
+  if (ensure_init()) return -1;
   preprocess_kernel<<<dim3((Wp + 31) / 32, (Hp + 7) / 8), dim3(32, 8), 0, static_cast<cudaStream_t>(stream)>>>(
       img_hwc, out, h, w, Ho, Wo, Hp, Wp, mean3_host[0], mean3_host[1], mean3_host[2], std3_host[0], std3_host[1],
       std3_host[2], pad3_host[0], pad3_host[1], pad3_host[2]);
@@ -1036,16 +1065,33 @@ int lseg_mhsa_trace(const void* qkv, void* out, int B, int N, int heads, int cau
 
 int lseg_layernorm(const void* x, int in_f16, const float* gamma, const float* beta, void* y, long long M, int C,
                    float eps, void* stream) {
+  const char* fn = "lseg_layernorm";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "gamma", gamma, 16) || arg_ptr(fn, "beta", beta, 16) ||
+      arg_ptr(fn, "y", y, 16) || arg_pos(fn, "M", M) || arg_max(fn, "M / 8 blocks", (M + 7) / 8, kGridX))
+    return -1;
+  if (C != 512 && C != 768 && C != 1024) return set_error("%s: C=%d must be 512, 768 or 1024", fn, C), -1;
   if (ensure_init()) return -1;
   return run_layernorm(x, in_f16, gamma, beta, static_cast<__half*>(y), M, C, eps, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_patchify(const float* x, void* a, int B, int H, int W, int patch, void* stream) {
+  const char* fn = "lseg_patchify";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "a", a, 8) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_pos(fn, "patch", patch) ||
+      arg_max(fn, "B*(H/patch)", static_cast<long long>(B) * (H / patch), kGridYZ))
+    return -1;
+  if (patch != 16 && patch != 32) return set_error("%s: patch=%d must be 16 or 32", fn, patch), -1;
+  if (arg_mult(fn, "H", H, patch) || arg_mult(fn, "W", W, patch)) return -1;
   if (ensure_init()) return -1;
   return launch_patchify(x, static_cast<__half*>(a), B, H, W, patch, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_pos_resize(const float* pos, float* out, int g0, int gh, int gw, int D, void* stream) {
+  const char* fn = "lseg_pos_resize";
+  if (arg_ptr(fn, "pos", pos, 4) || arg_ptr(fn, "out", out, 4) || arg_pos(fn, "g0", g0) || arg_pos(fn, "gh", gh) ||
+      arg_pos(fn, "gw", gw) || arg_pos(fn, "D", D) ||
+      arg_max(fn, "1 + gh*gw", 1 + static_cast<long long>(gh) * gw, kGridX))
+    return -1;
   if (ensure_init()) return -1;
   pos_resize_kernel<<<1 + gh * gw, 256, 0, static_cast<cudaStream_t>(stream)>>>(pos, out, g0, gh, gw, D);
   LSEG_CHECK_CUDA(cudaGetLastError());
@@ -1054,40 +1100,75 @@ int lseg_pos_resize(const float* pos, float* out, int g0, int gh, int gw, int D,
 
 int lseg_assemble_tokens(const float* patch, const float* cls, const float* pos, float* x, int B, int T, int D,
                          void* stream) {
+  const char* fn = "lseg_assemble_tokens";
+  if (arg_ptr(fn, "patch", patch, 16) || arg_ptr(fn, "cls", cls, 16) || arg_ptr(fn, "pos", pos, 16) ||
+      arg_ptr(fn, "x", x, 16) || arg_pos(fn, "B", B) || arg_pos(fn, "T", T) || arg_pos(fn, "D", D) ||
+      arg_mult(fn, "D", D, 4) || arg_max(fn, "B*(T+1)", static_cast<long long>(B) * (T + 1), kGridX))
+    return -1;
   if (ensure_init()) return -1;
   return launch_assemble_tokens(patch, cls, pos, x, B, T, D, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_readout_split(const float* tap, void* tok, void* cls, int B, int T, int D, void* stream) {
+  const char* fn = "lseg_readout_split";
+  if (arg_ptr(fn, "tap", tap, 16) || arg_ptr(fn, "tok", tok, 8) || arg_ptr(fn, "cls", cls, 8) || arg_pos(fn, "B", B) ||
+      arg_pos(fn, "T", T) || arg_pos(fn, "D", D) || arg_mult(fn, "D", D, 4) ||
+      arg_max(fn, "B*(T+1)", static_cast<long long>(B) * (T + 1), kGridX))
+    return -1;
   if (ensure_init()) return -1;
   return launch_readout_split(tap, static_cast<__half*>(tok), static_cast<__half*>(cls), B, T, D,
                               static_cast<cudaStream_t>(stream));
 }
 
 int lseg_im2col_3x3_s2(const void* x, void* a, int B, int H, int W, int C, void* stream) {
+  const char* fn = "lseg_im2col_3x3_s2";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "a", a, 16) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_pos(fn, "C", C) || arg_mult(fn, "C", C, 8) || arg_max(fn, "B", B, kGridYZ) ||
+      arg_max(fn, "Ho", (H - 1) / 2 + 1, kGridYZ))
+    return -1;
   if (ensure_init()) return -1;
   return launch_im2col_3x3_s2(static_cast<const __half*>(x), static_cast<__half*>(a), B, H, W, C,
                               static_cast<cudaStream_t>(stream));
 }
 
 int lseg_stem_im2col(const float* x, void* a, int B, int H, int W, void* stream) {
+  const char* fn = "lseg_stem_im2col";
+  if (arg_ptr(fn, "x", x, 4) || arg_ptr(fn, "a", a, 2) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_max(fn, "B*(H/2)*(W/2)", static_cast<long long>(B) * (H / 2) * (W / 2), kGridX) ||
+      arg_mult(fn, "H", H, 2) || arg_mult(fn, "W", W, 2))
+    return -1;
   if (ensure_init()) return -1;
   return launch_stem_im2col(x, static_cast<__half*>(a), B, H, W, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_maxpool3x3s2_nhwc(const void* x, void* y, int B, int H, int W, int C, void* stream) {
+  const char* fn = "lseg_maxpool3x3s2_nhwc";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_pos(fn, "C", C) || arg_max(fn, "B", B, kGridYZ) || arg_mult(fn, "C", C, 8) ||
+      arg_mult(fn, "H", H, 2) || arg_mult(fn, "W", W, 2))
+    return -1;
   if (ensure_init()) return -1;
   return launch_maxpool3x3s2_nhwc(static_cast<const __half*>(x), static_cast<__half*>(y), B, H, W, C,
                                   static_cast<cudaStream_t>(stream));
 }
 
 int lseg_subsample2_nhwc(const void* x, void* y, int B, int H, int W, int C, void* stream) {
+  const char* fn = "lseg_subsample2_nhwc";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_pos(fn, "C", C) || arg_max(fn, "B", B, kGridYZ) || arg_mult(fn, "C", C, 8) ||
+      arg_mult(fn, "H", H, 2) || arg_mult(fn, "W", W, 2))
+    return -1;
   if (ensure_init()) return -1;
   return launch_subsample2_nhwc(static_cast<const __half*>(x), static_cast<__half*>(y), B, H, W, C,
                                 static_cast<cudaStream_t>(stream));
 }
 
 int lseg_upsample2x_nhwc(const void* x, void* y, int B, int H, int W, int C, void* stream) {
+  const char* fn = "lseg_upsample2x_nhwc";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "B", B) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_pos(fn, "C", C) || arg_mult(fn, "C", C, 8) || arg_max(fn, "B", B, kGridYZ) ||
+      arg_max(fn, "2H", 2LL * H, kGridYZ))
+    return -1;
   if (ensure_init()) return -1;
   return launch_upsample2x_nhwc(static_cast<const __half*>(x), static_cast<__half*>(y), B, H, W, C,
                                 static_cast<cudaStream_t>(stream));
@@ -1095,11 +1176,13 @@ int lseg_upsample2x_nhwc(const void* x, void* y, int B, int H, int W, int C, voi
 
 int lseg_upsample2x_nhwc256(const void* x, int in_f16, void* y, int out_f16, const float* add, int B, int H, int W,
                             void* stream) {
-  if (ensure_init()) return -1;
-  if (add && out_f16) {
-    set_error("upsample2x_nhwc256: the skip operand goes with an fp32 output");
+  const char* fn = "lseg_upsample2x_nhwc256";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || (add && arg_ptr(fn, "add", add, 16)) ||
+      arg_pos(fn, "B", B) || arg_pos(fn, "H", H) || arg_pos(fn, "W", W) || arg_max(fn, "B", B, kGridYZ) ||
+      arg_max(fn, "2H", 2LL * H, kGridYZ))
     return -1;
-  }
+  if (ensure_init()) return -1;
+  if (add && out_f16) return set_error("%s: add (the skip operand) needs an fp32 output (out_f16=0)", fn), -1;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (in_f16) {
     if (out_f16) return launch_upsample2x_nhwc256_f16<__half>(static_cast<const __half*>(x), static_cast<__half*>(y), nullptr, B, H, W, s);
@@ -1110,11 +1193,11 @@ int lseg_upsample2x_nhwc256(const void* x, int in_f16, void* y, int out_f16, con
 }
 
 int lseg_l2norm_scale(const float* x, void* y, long long M, int C, float logit_scale, void* stream) {
-  if (ensure_init()) return -1;
-  if (C % 128 != 0 || C > 512) {
-    set_error("l2norm_scale: C=%d must be a multiple of 128 and <= 512", C);
+  const char* fn = "lseg_l2norm_scale";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 8) || arg_pos(fn, "M", M) || arg_pos(fn, "C", C) ||
+      arg_max(fn, "M / 8 blocks", (M + 7) / 8, kGridX) || arg_mult(fn, "C", C, 128) || arg_max(fn, "C", C, 512))
     return -1;
-  }
+  if (ensure_init()) return -1;
   const int grid = static_cast<int>((M + 7) / 8);
   l2norm_scale_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, static_cast<__half*>(y), M, C,
                                                                            logit_scale);
@@ -1123,6 +1206,8 @@ int lseg_l2norm_scale(const float* x, void* y, long long M, int C, float logit_s
 }
 
 int lseg_l2norm_f16(const void* x, void* y, int M, int C, void* stream) {
+  const char* fn = "lseg_l2norm_f16";
+  if (arg_ptr(fn, "x", x, 2) || arg_ptr(fn, "y", y, 2) || arg_pos(fn, "M", M) || arg_pos(fn, "C", C)) return -1;
   if (ensure_init()) return -1;
   l2norm_f16_kernel<<<(M + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const __half*>(x),
                                                                                static_cast<__half*>(y), M, C);
@@ -1131,11 +1216,11 @@ int lseg_l2norm_f16(const void* x, void* y, int M, int C, void* stream) {
 }
 
 int lseg_upsample2x_nchw(const void* x, float* y, long long planes, int H, int W, void* stream) {
-  if (ensure_init()) return -1;
-  if ((2 * W) % 4 != 0) {
-    set_error("upsample2x_nchw: output width must be a multiple of 4");
+  const char* fn = "lseg_upsample2x_nchw";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "planes", planes) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_up_w(fn, W) || arg_max(fn, "planes", planes, kGridYZ))
     return -1;
-  }
+  if (ensure_init()) return -1;
   return launch_upsample2x_nchw(static_cast<const __half*>(x), y, planes, H, W, static_cast<cudaStream_t>(stream));
 }
 
@@ -1146,26 +1231,34 @@ int lseg_debug_upsample_layout(int split) {
 }
 
 int lseg_upsample2x_nchw_bg(const void* x, float* y, long long planes, int H, int W, void* stream) {
+  const char* fn = "lseg_upsample2x_nchw_bg";
+  if (arg_ptr(fn, "x", x, 2) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "planes", planes) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_mult(fn, "W", W, 2) || arg_max(fn, "planes", planes, kGridYZ))
+    return -1;
   if (ensure_init()) return -1;
   return launch_upsample2x_nchw_bg(static_cast<const __half*>(x), y, planes, H, W, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_upsample2x_nchw_f32(const float* x, float* y, long long planes, int H, int W, void* stream) {
-  if (ensure_init()) return -1;
-  if ((2 * W) % 4 != 0) {
-    set_error("upsample2x_nchw: output width must be a multiple of 4");
+  const char* fn = "lseg_upsample2x_nchw_f32";
+  if (arg_ptr(fn, "x", x, 16) || arg_ptr(fn, "y", y, 16) || arg_pos(fn, "planes", planes) || arg_pos(fn, "H", H) ||
+      arg_pos(fn, "W", W) || arg_up_w(fn, W) || arg_max(fn, "planes", planes, kGridYZ))
     return -1;
-  }
+  if (ensure_init()) return -1;
   return launch_upsample2x_nchw(x, y, planes, H, W, static_cast<cudaStream_t>(stream));
 }
 
 int lseg_head_block(const void* x, int in_f16, float* cmax_ws, float* y, int B, int K, int h, int w, const float* w9_host,
                     float bias, int mode, int act, void* stream) {
-  if (ensure_init()) return -1;
-  if (!x || !y || !w9_host || (mode != 1 && mode != 2) || (mode == 1 && !cmax_ws)) {
-    set_error("lseg_head_block: bad argument");
+  const char* fn = "lseg_head_block";
+  if (arg_ptr(fn, "x", x, in_f16 ? 2 : 4) || arg_ptr(fn, "y", y, 4) || arg_ptr(fn, "w9", w9_host, 4)) return -1;
+  if (mode != 1 && mode != 2) return set_error("%s: mode=%d must be 1 or 2", fn, mode), -1;
+  if (act < HEAD_ACT_NONE || act > HEAD_ACT_TANH) return set_error("%s: act=%d must be 0..3", fn, act), -1;
+  if ((mode == 1 && arg_ptr(fn, "cmax_ws", cmax_ws, 4)) || arg_pos(fn, "B", B) || arg_pos(fn, "K", K) ||
+      arg_pos(fn, "h", h) || arg_pos(fn, "w", w) || arg_max(fn, "ceil(h/8)", (h + 7) / 8, kGridYZ) ||
+      arg_max(fn, "B", B, kGridYZ) || arg_max(fn, "B*K", static_cast<long long>(B) * K, kGridYZ))
     return -1;
-  }
+  if (ensure_init()) return -1;
   HeadBlockW hw;
   for (int i = 0; i < 9; ++i) hw.w[i] = w9_host[i];
   hw.bias = bias;
@@ -1177,6 +1270,10 @@ int lseg_head_block(const void* x, int in_f16, float* cmax_ws, float* y, int B, 
 }
 
 int lseg_upsample2x_argmax(const void* lr, long long* mask, int B, int K, int H, int W, void* stream) {
+  const char* fn = "lseg_upsample2x_argmax";
+  if (arg_ptr(fn, "lr", lr, 16) || arg_ptr(fn, "mask", mask, 8) || arg_pos(fn, "B", B) || arg_pos(fn, "K", K) ||
+      arg_pos(fn, "H", H) || arg_pos(fn, "W", W) || arg_up_w(fn, W) || arg_max(fn, "B", B, kGridYZ))
+    return -1;
   if (ensure_init()) return -1;
   return launch_upsample2x_argmax(static_cast<const __half*>(lr), mask, B, K, H, W, static_cast<cudaStream_t>(stream));
 }
@@ -1197,6 +1294,11 @@ int lseg_seg_stats_mask(const long long* pred, const long long* target, const in
 
 int lseg_text_embed(const int64_t* tokens, const float* tok_emb, const float* pos_emb, void* x, int K, int L, int Wd,
                     void* stream) {
+  const char* fn = "lseg_text_embed";
+  if (arg_ptr(fn, "tokens", tokens, 8) || arg_ptr(fn, "tok_emb", tok_emb, 4) || arg_ptr(fn, "pos_emb", pos_emb, 4) ||
+      arg_ptr(fn, "x", x, 2) || arg_pos(fn, "K", K) || arg_pos(fn, "L", L) || arg_pos(fn, "Wd", Wd) ||
+      arg_max(fn, "K*L", static_cast<long long>(K) * L, kGridX))
+    return -1;
   if (ensure_init()) return -1;
   text_embed_kernel<<<K * L, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(tokens), tok_emb, pos_emb, static_cast<__half*>(x), L, Wd);
@@ -1205,6 +1307,10 @@ int lseg_text_embed(const int64_t* tokens, const float* tok_emb, const float* po
 }
 
 int lseg_text_eot_gather(const int64_t* tokens, const void* x, void* out, int K, int L, int Wd, void* stream) {
+  const char* fn = "lseg_text_eot_gather";
+  if (arg_ptr(fn, "tokens", tokens, 8) || arg_ptr(fn, "x", x, 2) || arg_ptr(fn, "out", out, 2) || arg_pos(fn, "K", K) ||
+      arg_pos(fn, "L", L) || arg_pos(fn, "Wd", Wd))
+    return -1;
   if (ensure_init()) return -1;
   text_eot_gather_kernel<<<K, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const long long*>(tokens), static_cast<const __half*>(x), static_cast<__half*>(out), K, L, Wd);

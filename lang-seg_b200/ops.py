@@ -29,6 +29,18 @@ def _ptr(t, dtype=None):
     return C.c_void_p(t.data_ptr())
 
 
+def _out(out, shape, dtype, device, what):
+    """The output buffer of a glue op: a fresh torch.empty, or the caller's tensor, which must be exactly a contiguous
+    `dtype` tensor of `shape` on `device` (the kernels write that many elements through a raw pointer, unchecked)."""
+    shape = tuple(int(v) for v in shape)
+    if out is None:
+        return torch.empty(shape, dtype=dtype, device=device)
+    if out.dtype != dtype or tuple(out.shape) != shape or out.device != torch.device(device) or not out.is_contiguous():
+        raise _lib.LsegError(f"{what}: out must be a contiguous {dtype} {list(shape)} tensor on {device}, got "
+                             f"{out.dtype} {list(out.shape)} on {out.device}{'' if out.is_contiguous() else ' (strided)'}")
+    return out
+
+
 def pad_rows(w, mult=128):
     """Weights are [N, K] fp16 with rows padded to a multiple of 128 (TMA box never exceeds the tensor)."""
     n = w.shape[0]
@@ -163,10 +175,11 @@ def text_attn(qkv, K, L, heads, out=None):
     return out
 
 
-def head_block(x, weight9, bias, mode, act):
-    """One application of scratch.head_block on x [B,K,h,w] (fp16 or fp32) -> fp32 (include/lseg_b200.h lseg_head_block)."""
+def head_block(x, weight9, bias, mode, act, out=None):
+    """One application of scratch.head_block on x [B,K,h,w] (fp16 or fp32) -> fp32 (include/lseg_b200.h lseg_head_block).
+    out: optional contiguous fp32 [B,K,h,w]."""
     B, K, h, w = x.shape
-    y = torch.empty((B, K, h, w), dtype=torch.float32, device=x.device)
+    y = _out(out, (B, K, h, w), torch.float32, x.device, "head_block")
     cmax = torch.empty((B, h, w), dtype=torch.float32, device=x.device)
     w9 = (C.c_float * 9)(*[float(v) for v in weight9])
     check(load().lseg_head_block(_ptr(x), int(x.dtype == torch.float16), _ptr(cmax), _ptr(y), B, K, h, w, w9, float(bias),
@@ -174,15 +187,15 @@ def head_block(x, weight9, bias, mode, act):
     return y
 
 
-def upsample2x_nchw_f32(x):
+def upsample2x_nchw_f32(x, out=None):
     planes = x.numel() // (x.shape[-1] * x.shape[-2])
     H, W = x.shape[-2:]
-    y = torch.empty(tuple(x.shape[:-2]) + (2 * H, 2 * W), dtype=torch.float32, device=x.device)
+    y = _out(out, tuple(x.shape[:-2]) + (2 * H, 2 * W), torch.float32, x.device, "upsample2x_nchw_f32")
     check(load().lseg_upsample2x_nchw_f32(_ptr(x, torch.float32), _ptr(y), planes, H, W, _stream()))
     return y
 
 
-def preprocess(img_u8, size, pad_to=None, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5)):
+def preprocess(img_u8, size, pad_to=None, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5), out=None):
     """uint8 HWC image on the GPU -> fp32 [1,3,Hp,Wp]: ToTensor + Normalize + Resize(size) (bilinear, align_corners=False,
     no antialias: torchvision's tensor resize of the reference's era) + constant pad with -mean/std (pad_image) to
     `pad_to`. One kernel (include/lseg_b200.h lseg_preprocess; lseg_app.py:328-334)."""
@@ -191,7 +204,7 @@ def preprocess(img_u8, size, pad_to=None, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0
     h, w = img_u8.shape[:2]
     Ho, Wo = size
     Hp, Wp = pad_to if pad_to is not None else (Ho, Wo)
-    out = torch.empty((1, 3, Hp, Wp), dtype=torch.float32, device=img_u8.device)
+    out = _out(out, (1, 3, Hp, Wp), torch.float32, img_u8.device, "preprocess")
     m3 = (C.c_float * 3)(*[float(v) for v in mean])
     s3 = (C.c_float * 3)(*[float(v) for v in std])
     p3 = (C.c_float * 3)(*[-float(a) / float(b) for a, b in zip(mean, std)])
@@ -213,80 +226,86 @@ def mhsa_trace(qkv, B, N, heads, causal=False, out=None):
     return out, trace
 
 
-def layernorm(x, gamma, beta, eps):
+def layernorm(x, gamma, beta, eps, out=None):
     M, Cc = x.shape
-    y = torch.empty((M, Cc), dtype=torch.float16, device=x.device)
+    y = _out(out, (M, Cc), torch.float16, x.device, "layernorm")
     check(load().lseg_layernorm(_ptr(x), int(x.dtype == torch.float16), _ptr(gamma, torch.float32),
                                 _ptr(beta, torch.float32), _ptr(y), M, Cc, eps, _stream()))
     return y
 
 
-def patchify(x, patch=16):
+def patchify(x, patch=16, out=None):
     B, _, H, W = x.shape
-    a = torch.empty((B * (H // patch) * (W // patch), 3 * patch * patch), dtype=torch.float16, device=x.device)
+    a = _out(out, (B * (H // patch) * (W // patch), 3 * patch * patch), torch.float16, x.device, "patchify")
     check(load().lseg_patchify(_ptr(x, torch.float32), _ptr(a), B, H, W, patch, _stream()))
     return a
 
 
-def pos_resize(pos, g0, gh, gw):
+def pos_resize(pos, g0, gh, gw, out=None):
     D = pos.shape[-1]
-    out = torch.empty((1 + gh * gw, D), dtype=torch.float32, device=pos.device)
+    out = _out(out, (1 + gh * gw, D), torch.float32, pos.device, "pos_resize")
     check(load().lseg_pos_resize(_ptr(pos, torch.float32), _ptr(out), g0, gh, gw, D, _stream()))
     return out
 
 
-def assemble_tokens(patch, cls, pos, B, T):
+def assemble_tokens(patch, cls, pos, B, T, out=None):
     D = patch.shape[-1]
-    x = torch.empty((B, T + 1, D), dtype=torch.float32, device=patch.device)
+    x = _out(out, (B, T + 1, D), torch.float32, patch.device, "assemble_tokens")
     check(load().lseg_assemble_tokens(_ptr(patch, torch.float32), _ptr(cls, torch.float32), _ptr(pos, torch.float32),
                                       _ptr(x), B, T, D, _stream()))
     return x
 
 
-def readout_split(tap):
+def readout_split(tap, out=None):
+    """tap fp32 [B, N, D] -> (tok fp16 [B*(N-1), D], cls fp16 [B rounded up to 128, D]); the kernel writes cls rows < B
+    only, the padding rows stay as the caller left them (zero when allocated here). out: optional (tok, cls) pair."""
     B, N, D = tap.shape
-    tok = torch.empty((B * (N - 1), D), dtype=torch.float16, device=tap.device)
-    cls = torch.zeros(((B + 127) // 128 * 128, D), dtype=torch.float16, device=tap.device)
+    tok_out, cls_out = out if out is not None else (None, None)
+    tok = _out(tok_out, (B * (N - 1), D), torch.float16, tap.device, "readout_split tok")
+    if cls_out is None:
+        cls = torch.zeros(((B + 127) // 128 * 128, D), dtype=torch.float16, device=tap.device)
+    else:
+        cls = _out(cls_out, ((B + 127) // 128 * 128, D), torch.float16, tap.device, "readout_split cls")
     check(load().lseg_readout_split(_ptr(tap, torch.float32), _ptr(tok), _ptr(cls), B, N - 1, D, _stream()))
     return tok, cls
 
 
-def im2col_3x3_s2(x):
+def im2col_3x3_s2(x, out=None):
     B, H, W, Cc = x.shape
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-    a = torch.empty((B * Ho * Wo, 9 * Cc), dtype=torch.float16, device=x.device)
+    a = _out(out, (B * Ho * Wo, 9 * Cc), torch.float16, x.device, "im2col_3x3_s2")
     check(load().lseg_im2col_3x3_s2(_ptr(x, torch.float16), _ptr(a), B, H, W, Cc, _stream()))
     return a
 
 
-def stem_im2col(x):
+def stem_im2col(x, out=None):
     """x fp32 NCHW [B,3,H,W] -> fp16 [B*(H/2)*(W/2), 192] rows of the ResNet stem conv (7x7 s2 p3), zero beyond column 147."""
     B, _, H, W = x.shape
-    a = torch.empty((B * (H // 2) * (W // 2), 192), dtype=torch.float16, device=x.device)
+    a = _out(out, (B * (H // 2) * (W // 2), 192), torch.float16, x.device, "stem_im2col")
     check(load().lseg_stem_im2col(_ptr(x, torch.float32), _ptr(a), B, H, W, _stream()))
     return a
 
 
-def maxpool3x3s2_nhwc(x):
+def maxpool3x3s2_nhwc(x, out=None):
     B, H, W, Cc = x.shape
-    y = torch.empty((B, H // 2, W // 2, Cc), dtype=torch.float16, device=x.device)
+    y = _out(out, (B, H // 2, W // 2, Cc), torch.float16, x.device, "maxpool3x3s2_nhwc")
     check(load().lseg_maxpool3x3s2_nhwc(_ptr(x, torch.float16), _ptr(y), B, H, W, Cc, _stream()))
     return y
 
 
-def subsample2_nhwc(x):
+def subsample2_nhwc(x, out=None):
     B, H, W, Cc = x.shape
-    y = torch.empty((B, H // 2, W // 2, Cc), dtype=torch.float16, device=x.device)
+    y = _out(out, (B, H // 2, W // 2, Cc), torch.float16, x.device, "subsample2_nhwc")
     check(load().lseg_subsample2_nhwc(_ptr(x, torch.float16), _ptr(y), B, H, W, Cc, _stream()))
     return y
 
 
-def upsample2x_nhwc(x, out_dtype=torch.float16, add=None, decoder=False):
+def upsample2x_nhwc(x, out_dtype=torch.float16, add=None, decoder=False, out=None):
     """bilinear x2 align_corners=True over NHWC. decoder=False: the generic fp16 -> fp16 kernel (any C);
     decoder=True (or fp32 input / fp32 output / add): the C = 256 kernels of the fusion blocks — fp16 | fp32 source,
     fp16 | fp32 result, optional fp32 skip operand summed in."""
     B, H, W, Cc = x.shape
-    y = torch.empty((B, 2 * H, 2 * W, Cc), dtype=out_dtype, device=x.device)
+    y = _out(out, (B, 2 * H, 2 * W, Cc), out_dtype, x.device, "upsample2x_nhwc")
     if decoder or x.dtype == torch.float32 or out_dtype == torch.float32 or add is not None:
         if Cc != 256:
             raise ValueError("the decoder interpolation kernels are built for C = 256")
@@ -298,24 +317,24 @@ def upsample2x_nhwc(x, out_dtype=torch.float16, add=None, decoder=False):
     return y
 
 
-def l2norm_scale(x, logit_scale):
+def l2norm_scale(x, logit_scale, out=None):
     M, Cc = x.shape
-    y = torch.empty((M, Cc), dtype=torch.float16, device=x.device)
+    y = _out(out, (M, Cc), torch.float16, x.device, "l2norm_scale")
     check(load().lseg_l2norm_scale(_ptr(x, torch.float32), _ptr(y), M, Cc, float(logit_scale), _stream()))
     return y
 
 
-def l2norm_f16(x):
+def l2norm_f16(x, out=None):
     M, Cc = x.shape
-    y = torch.empty_like(x)
+    y = _out(out, (M, Cc), torch.float16, x.device, "l2norm_f16")
     check(load().lseg_l2norm_f16(_ptr(x, torch.float16), _ptr(y), M, Cc, _stream()))
     return y
 
 
-def upsample2x_nchw(x, background=False):
+def upsample2x_nchw(x, background=False, out=None):
     """background=True: the shared-memory-free kernel of the multi-GPU gather (same values bit for bit)."""
     B, K, H, W = x.shape
-    y = torch.empty((B, K, 2 * H, 2 * W), dtype=torch.float32, device=x.device)
+    y = _out(out, (B, K, 2 * H, 2 * W), torch.float32, x.device, "upsample2x_nchw")
     fn = load().lseg_upsample2x_nchw_bg if background else load().lseg_upsample2x_nchw
     check(fn(_ptr(x, torch.float16), _ptr(y), B * K, H, W, _stream()))
     return y
@@ -373,19 +392,23 @@ def seg_stats_mask(pred, target, stats, nclass, group=None):
     return stats
 
 
-def text_embed(tokens, tok_emb, pos_emb):
+def text_embed(tokens, tok_emb, pos_emb, out=None):
     K, L = tokens.shape
     Wd = tok_emb.shape[1]
-    x = torch.empty((K * L, Wd), dtype=torch.float16, device=tok_emb.device)
+    x = _out(out, (K * L, Wd), torch.float16, tok_emb.device, "text_embed")
     check(load().lseg_text_embed(_ptr(tokens, torch.int64), _ptr(tok_emb, torch.float32),
                                  _ptr(pos_emb, torch.float32), _ptr(x), K, L, Wd, _stream()))
     return x
 
 
-def text_eot_gather(tokens, x):
+def text_eot_gather(tokens, x, out=None):
+    """Rows [K rounded up to 128, Wd]: the kernel writes rows < K, the padding rows stay as the caller left them."""
     K, L = tokens.shape
     Wd = x.shape[-1]
-    out = torch.zeros(((K + 127) // 128 * 128, Wd), dtype=torch.float16, device=x.device)
+    if out is None:
+        out = torch.zeros(((K + 127) // 128 * 128, Wd), dtype=torch.float16, device=x.device)
+    else:
+        out = _out(out, ((K + 127) // 128 * 128, Wd), torch.float16, x.device, "text_eot_gather")
     check(load().lseg_text_eot_gather(_ptr(tokens, torch.int64), _ptr(x, torch.float16), _ptr(out), K, L, Wd,
                                       _stream()))
     return out

@@ -11,9 +11,11 @@
 //   warpgroup 0   TMA producer (warp 0, one elected lane; 24 registers): fills the A/B smem ring (128B-swizzled,
 //                 K-major) in list order
 //   warpgroups 1-2  consumers (240 registers): the list's entries alternate between them. A warpgroup computes its whole
-//                 tile (two wgmma m64n128k16 per k16 step, 2 x 64 fp32 accumulators per thread), then stages it in its
-//                 own shared-memory area one 64-column half at a time, and its 4 warps run the epilogue with thread <->
-//                 output row (warp = 32 rows x 64 columns per half): scale/bias/act/residual -> global.
+//                 tile (two wgmma m64n128k16 per k16 step, 2 x 64 fp32 accumulators per thread), then runs its epilogue:
+//                 the TMA epilogues straight from each warp's accumulator fragment (gemm_epilogue_frag); the register-
+//                 direct one, and the fp16 TMA store of GEMMs with row sums, stage the tile in the warpgroup's own
+//                 shared-memory area one 64-column half at a time and map thread <-> output row (warp = 32 rows x 64
+//                 columns per half): scale/bias/act/residual -> global.
 // The MMA turn passes from one warpgroup to the other in list order (named barriers), so one warpgroup's epilogue
 // runs while the other's MMAs keep the tensor cores busy; the tensor pipe idles only where an epilogue takes longer
 // than a main loop, or where a CTA owns a single tile. The accumulation order of every output element (the same
@@ -21,14 +23,18 @@
 // Grids with more work units than SMs and an even n-tile count run as 2-CTA clusters that share the A tile (CLUSTER,
 // see the kernel); lseg_b200.cu (gemm_plan_grid) has the rule and the numbers behind it.
 // Measured (B=8, 480x480, H100 80GB HBM3 SXM at a 700 W power limit, tools/gemm_shapes.py, as planned): ViT linears
-// 480-510 TFLOP/s (QKV, fc1) and 340-400 (proj, fc2); 3x3 decoder convs 320-480 at 60^2 / 120^2; head1 280.
+// 530-600 TFLOP/s (QKV, fc1) and 350-490 (proj, fc2); 3x3 decoder convs 320-480 at 60^2 / 120^2; head1 (staged row-sum
+// form) 290-300.
 //
 // Epilogue modes:
 //   EPI_DIRECT   stores straight from registers, thread <-> accumulator row.
-//   EPI_TMA_F16  fp16 row-major outputs: each epilogue warp packs 32 rows x 64 columns into a private
-//                128B-swizzled smem tile and one elected lane issues a bulk tensor store.
-//   EPI_TMA_ADD  in-place fp32 residual stream (x += A W^T + b): the warp stages 32 x 32 fp32 results and
+//   EPI_TMA_F16  fp16 row-major outputs: each warp converts its own fragment rows (16 per m64 half) and packs 16 rows x
+//                64 columns into a private 128B-swizzled smem box; one elected lane issues a bulk tensor store.
+//   EPI_TMA_ADD  in-place fp32 residual stream (x += A W^T + b): the warp packs 16 x 32 fp32 results the same way and
 //                issues a bulk tensor REDUCE-ADD, so the residual is never read by the SM at all.
+//   The TMA epilogues need no accumulator staging area and no warpgroup barrier, so their operand ring has 6 stages
+//   (register-direct: 5). Exception: EPI_TMA_F16 plans with row sums (head1's out_row_sumsq, summed per row in column
+//   order) run the staged form EPI_TMA_F16_STAGED (4 stages, gemm_tma_f16_staged), where a thread holds whole rows.
 // Per-column constants (bias, folded-BN scale) live in registers per tile and are distributed by shuffle.
 #pragma once
 #include "common.cuh"
@@ -43,7 +49,9 @@ constexpr int kConvTW = 16;
 
 enum GemmAct { ACT_NONE = 0, ACT_GELU = 1, ACT_QUICKGELU = 2, ACT_RELU = 3 };
 enum GemmStore { STORE_ROWMAJOR = 0, STORE_D2S = 1, STORE_NCHW_T = 2 };
-enum GemmEpiMode { EPI_DIRECT = 0, EPI_TMA_F16 = 1, EPI_TMA_ADD = 2 };
+// EPI_TMA_F16_STAGED is no plan's mode but a kernel form: the EPI_TMA_F16 plans with row sums (out_row_sumsq) run the
+// fp16 TMA store through the staged accumulators (gemm_tma_f16_staged).
+enum GemmEpiMode { EPI_DIRECT = 0, EPI_TMA_F16 = 1, EPI_TMA_ADD = 2, EPI_TMA_F16_STAGED = 3 };
 
 struct GemmEpi {
   const float* bias;       // [N] (or [groups, N] when bias_group_rows > 0); nullable
@@ -73,8 +81,9 @@ struct GemmEpi {
 struct GemmParams {
   CUtensorMap tma_a;  // plain: 2-D {K, M}; conv: 4-D {C, W, H, B}
   CUtensorMap tma_b;  // 2-D {Ktot, N}, Ktot = taps * C, tap-major
-  CUtensorMap tma_c;  // output map of the TMA epilogues. EPI_TMA_F16: fp16, plain 2-D {N, M} box {64, 32} /
-                      // conv 4-D {N, W, H, B} box {64, 16, 2, 1}. EPI_TMA_ADD: fp32 2-D {N, M} box {32, 32}.
+  CUtensorMap tma_c;  // output map of the TMA epilogues, one box = one warp's 16 fragment rows. EPI_TMA_F16: fp16, plain
+                      // 2-D {N, M} box {64, 16} / conv 4-D {N, W, H, B} box {64, 16, 1, 1}. EPI_TMA_ADD: fp32 2-D {N, M}
+                      // box {32, 16}.
                       // The map clips the M / H / W / N tails, so partial tiles need no masking.
   int M, N;
   int k_iters;   // total K chunks of 64 (taps * C/64)
@@ -431,160 +440,293 @@ __device__ __forceinline__ void gemm_acc_ld32(const float* acc_row, int c, int r
   }
 }
 
-// Epilogue of one 128 x (ncols) accumulator slab for one warp (r = quarter*32 + lane = this thread's row); acc_row is
-// this thread's row of the staged accumulators (gemm_acc_ld32), whose column 0 is output column n_base.
-// SINGLE_BUF: one 4 KB staging tile per warp instead of two (leaves the shared memory to the accumulator tile and the
-// operand ring; the warp then waits for its previous bulk store to finish reading before it refills the buffer).
+// Register-direct epilogue of one 128 x (ncols) accumulator slab for one warp (r = quarter*32 + lane = this thread's
+// row); acc_row is this thread's row of the staged accumulators (gemm_acc_ld32), whose column 0 is output column n_base.
 // RAGGED: the tile belongs to an image with rag_k labels whose first output plane is rag_koff (gemm_epilogue_store); its
 // column count takes the place of p.N.
-template <int EPI, bool SINGLE_BUF = false, bool GROUPED = false, bool RELU_RES = false, bool RAGGED = false,
-          typename WaitFn>
+template <bool GROUPED = false, bool RELU_RES = false, bool RAGGED = false, typename WaitFn>
 __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const float* acc_row, int n_base, int ncols,
-                                                   int m_tile, int r, WaitFn wait_accumulator, uint8_t* stage_buf,
-                                                   int& store_groups, GemmTrace& tr, bool first_k = true,
-                                                   int split_seg = 0, int rag_k = 0, int rag_koff = 0) {
+                                                   int m_tile, int r, WaitFn wait_accumulator, int split_seg = 0,
+                                                   int rag_k = 0, int rag_koff = 0) {
   const GemmEpi& e = p.e;
   long long grow;
   const bool valid = gemm_row_map(p, m_tile, r, grow);
   // split_fixed: this segment's plane of the partial-sum workspace (split_rows is 0 otherwise)
-  if constexpr (EPI == EPI_DIRECT) grow += split_seg * p.split_rows;
-  if constexpr (EPI == EPI_DIRECT) {
-    const int& N = RAGGED ? rag_k : p.N;  // plain lists: p.N itself (a parameter-space operand, as before)
-    // The fp32 residual of chunk c+1 is requested before chunk c is processed, and that of chunk 0 before the
-    // accumulator is even ready, so the residual read latency overlaps the main loop / the previous chunk.
-    const bool pre = valid && e.res_f32 && (e.store == STORE_ROWMAJOR);
-    const long long bias_off =
-        (e.bias_group_rows > 0 && valid) ? (grow / e.bias_group_rows) * static_cast<long long>(N) : 0;
-    float4 rnext[8];
+  grow += split_seg * p.split_rows;
+  const int& N = RAGGED ? rag_k : p.N;  // plain lists: p.N itself (a parameter-space operand, as before)
+  // The fp32 residual of chunk c+1 is requested before chunk c is processed, and that of chunk 0 before the
+  // accumulator is even ready, so the residual read latency overlaps the main loop / the previous chunk.
+  const bool pre = valid && e.res_f32 && (e.store == STORE_ROWMAJOR);
+  const long long bias_off =
+      (e.bias_group_rows > 0 && valid) ? (grow / e.bias_group_rows) * static_cast<long long>(N) : 0;
+  float4 rnext[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) rnext[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (pre && n_base + 32 <= N) {
-      const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n_base);
+  for (int j = 0; j < 8; ++j) rnext[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (pre && n_base + 32 <= N) {
+    const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n_base);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) rnext[j] = rp[j];
+  }
+  const GemmColConst cc = gemm_col_const(e, N, n_base, ncols, r & 31);
+  float row_mul = 1.f;
+  if (e.row_sumsq && valid) {  // deferred pixel normalisation: logit_scale / ||feature row||, once per tile
+    float ss = 0.f;
+    const float* sp = e.row_sumsq + grow * e.row_sumsq_parts;
+    for (int i = 0; i < e.row_sumsq_parts; ++i) ss += __ldg(sp + i);
+    row_mul = e.row_scale * rsqrtf(ss);
+  }
+  wait_accumulator();
+  if (p.probe & 1) return;
+#pragma unroll 1
+  for (int c = 0; c < ncols / 32; ++c) {
+    const int n0 = n_base + c * 32;
+    if (n0 >= N) break;  // warp-uniform
+    float4 rcur[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
+    const bool has_res = pre && (n0 + 32 <= N);
+    if (pre && (c + 1) * 32 < ncols && n0 + 64 <= N) {
+      const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n0 + 32);
 #pragma unroll
       for (int j = 0; j < 8; ++j) rnext[j] = rp[j];
     }
-    const GemmColConst cc = gemm_col_const(e, N, n_base, ncols, r & 31);
-    float row_mul = 1.f;
-    if (e.row_sumsq && valid) {  // deferred pixel normalisation: logit_scale / ||feature row||, once per tile
-      float ss = 0.f;
-      const float* sp = e.row_sumsq + grow * e.row_sumsq_parts;
-      for (int i = 0; i < e.row_sumsq_parts; ++i) ss += __ldg(sp + i);
-      row_mul = e.row_scale * rsqrtf(ss);
+    uint32_t v[32];
+    __syncwarp();
+    gemm_acc_ld32(acc_row, c, r, v);
+    float f[32];
+    gemm_epilogue_math(e, N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
+    if (valid) {
+      if (e.row_sumsq) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) f[i] *= row_mul;
+      }
+      gemm_epilogue_store<GROUPED, RELU_RES, RAGGED>(e, N, f, rcur, has_res, grow, n0, rag_koff);
     }
-    wait_accumulator();
-    if (p.probe & 1) return;
+  }
+}
+
+// fp16 TMA store of one 128 x (ncols) staged accumulator slab for one warp (thread <-> row r = quarter*32 + lane, as in
+// gemm_epilogue_tile), for the EPI_TMA_F16 plans with row sums: gemm_epilogue_math sums each row's 32-column chunks in
+// column order from the thread's own row. The warp packs 32 rows x 64 columns into its 4 KB 128B-swizzled staging tile
+// (waiting until its previous bulk store has read it) and the elected lane issues the store: tensor-map box {64, 32},
+// or {64, 16, 2, 1} for a conv.
+__device__ __forceinline__ void gemm_tma_f16_staged(const GemmParams& p, const float* acc_row, int n_base, int ncols,
+                                                    int m_tile, int r, uint8_t* stage_buf, int& store_groups,
+                                                    bool leader, GemmTrace& tr) {
+  const GemmEpi& e = p.e;
+  long long grow;
+  const bool valid = gemm_row_map(p, m_tile, r, grow);
+  const int lane = r & 31, quarter = r >> 5;
+  const long long grow_c = valid ? grow : 0;  // keep per-row lookups in range; the tensor map clips the rest
+  const long long bias_off = (e.bias_group_rows > 0) ? (grow_c / e.bias_group_rows) * static_cast<long long>(p.N) : 0;
+  int crd_w = 0, crd_h = 0, crd_b = 0;
+  if (p.conv) {
+    const int per_img = p.tiles_h * p.tiles_w;
+    crd_b = m_tile / per_img;
+    const int t = m_tile % per_img;
+    crd_h = (t / p.tiles_w) * kConvTH + quarter * 2;
+    crd_w = (t % p.tiles_w) * kConvTW;
+  }
+  const GemmColConst cc = gemm_col_const(e, p.N, n_base, ncols, lane);
+  tr(1);
+  if (p.probe & 1) return;
+  int groups = store_groups;
 #pragma unroll 1
-    for (int c = 0; c < ncols / 32; ++c) {
-      const int n0 = n_base + c * 32;
-      if (n0 >= N) break;  // warp-uniform
-      float4 rcur[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) rcur[j] = rnext[j];
-      const bool has_res = pre && (n0 + 32 <= N);
-      if (pre && (c + 1) * 32 < ncols && n0 + 64 <= N) {
-        const float4* rp = reinterpret_cast<const float4*>(e.res_f32 + grow * e.ldc + n0 + 32);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) rnext[j] = rp[j];
-      }
-      uint32_t v[32];
+  for (int c = 0; c < ncols / 32; ++c) {
+    const int n0 = n_base + c * 32;
+    if (n0 >= p.N) break;  // warp-uniform
+    uint32_t v[32];
+    __syncwarp();
+    gemm_acc_ld32(acc_row, c, r, v);
+    tr(2);
+    float f[32];
+    gemm_epilogue_math(e, p.N, v, grow_c, n0, bias_off, valid, f, cc, c);
+    tr(3);
+    if ((c & 1) == 0 && groups >= 1) {  // the previous bulk store must be done READING the staging tile
+      if (leader) tma_store_wait_read<0>();
       __syncwarp();
-      gemm_acc_ld32(acc_row, c, r, v);
-      float f[32];
-      gemm_epilogue_math(e, N, v, grow, n0, bias_off, valid, f, cc, c);  // all lanes: it shuffles
-      if (valid) {
-        if (e.row_sumsq) {
+    }
+    tr(4);
+    // 32 rows x 64 fp16 columns per group: this chunk fills 16-byte slots (c&1)*4 .. +3 of the row
 #pragma unroll
-          for (int i = 0; i < 32; ++i) f[i] *= row_mul;
-        }
-        gemm_epilogue_store<GROUPED, RELU_RES, RAGGED>(e, N, f, rcur, has_res, grow, n0, rag_koff);
+    for (int t = 0; t < 4; ++t) {
+      __half2 h[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(f[8 * t + 2 * i], f[8 * t + 2 * i + 1]);
+      const int slot = ((c & 1) * 4 + t) ^ (lane & 7);
+      *reinterpret_cast<uint4*>(stage_buf + lane * 128 + slot * 16) = *reinterpret_cast<uint4*>(h);
+    }
+    tr(5);
+    if ((c & 1) == 1 || c + 1 == ncols / 32 || n0 + 32 >= p.N) {
+      fence_proxy_async_smem();
+      __syncwarp();
+      const int col0 = n_base + (c & ~1) * 32;
+      if (leader) {
+        if (p.conv)
+          tma_store_4d(&p.tma_c, stage_buf, col0, crd_w, crd_h, crd_b);
+        else
+          tma_store_2d(&p.tma_c, stage_buf, col0, m_tile * kGemmBM + quarter * 32);
+        tma_store_commit();
+      }
+      ++groups;
+      tr(6);
+    }
+  }
+  store_groups = groups;
+}
+
+// TMA epilogues, straight from one warp's wgmma fragments. acc0 / acc1 hold tile rows 64 h + 16 wl + lane / 4 (acc[4 j],
+// acc[4 j + 1]) and + 8 (acc[4 j + 2], acc[4 j + 3]) of m64 half h = 0 / 1, columns 8 j + 2 (lane % 4) and + 1 (j = 0 .. 15;
+// column 0 = output column n_base). Row slot s = 2 h + t is the thread's row 64 h + 16 wl + lane / 4 + 8 t.
+// Each element gets gemm_epilogue_math's arithmetic in its order (scale, bias unless a stream-K segment starts past k = 0,
+// activation) with the same column constants (zero beyond N), so the results are those of the register-direct path.
+// The warp's 16 rows of a half leave in tensor-map boxes of 16 rows x 128 B: 64 fp16 columns (EPI_TMA_F16; a conv box is
+// one pixel row of the 8 x 16 tile), or 32 fp32 columns reduce-added into the residual stream (EPI_TMA_ADD). A box is
+// written into one of the warp's two 128B-swizzled staging buffers (bufs, 2 x 2 KB, 1024 B aligned), and the elected lane
+// issues the bulk op; before a buffer is refilled, the bulk op that last read it must be done reading. The tensor map
+// clips the M / H / W / N tails.
+
+// scale, bias and activation of one m64 half (row slots 2 h, 2 h + 1). sv / bv: the non-grouped column constants, lane l
+// holding columns 2 l, 2 l + 1 (index 0) and 64 + 2 l, + 1 (index 1) of the tile; column group j takes them from lane
+// 4 (j % 8) + lane % 4 by shuffle. A per-image bias depends on the row: each row slot loads its 16 pairs at once. Multiply
+// and add stay separate roundings (__fmul_rn / __fadd_rn), as in gemm_epilogue_math.
+__device__ __forceinline__ void gemm_frag_math(const GemmParams& p, float (&acc)[64], int h, int m_tile, int n_base,
+                                               int wl, int lane, const float2 (&sv)[2], const float2 (&bv)[2],
+                                               bool use_bias) {
+  const GemmEpi& e = p.e;
+  const int N = p.N;
+  const int q = lane & 3;
+  if (e.scale) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int src = 4 * (j & 7) + q;
+      const float sx = __shfl_sync(0xffffffffu, sv[j >> 3].x, src), sy = __shfl_sync(0xffffffffu, sv[j >> 3].y, src);
+      acc[4 * j] = __fmul_rn(acc[4 * j], sx);
+      acc[4 * j + 1] = __fmul_rn(acc[4 * j + 1], sy);
+      acc[4 * j + 2] = __fmul_rn(acc[4 * j + 2], sx);
+      acc[4 * j + 3] = __fmul_rn(acc[4 * j + 3], sy);
+    }
+  }
+  if (use_bias && e.bias_group_rows == 0) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int src = 4 * (j & 7) + q;
+      const float bx = __shfl_sync(0xffffffffu, bv[j >> 3].x, src), by = __shfl_sync(0xffffffffu, bv[j >> 3].y, src);
+      acc[4 * j] = __fadd_rn(acc[4 * j], bx);
+      acc[4 * j + 1] = __fadd_rn(acc[4 * j + 1], by);
+      acc[4 * j + 2] = __fadd_rn(acc[4 * j + 2], bx);
+      acc[4 * j + 3] = __fadd_rn(acc[4 * j + 3], by);
+    }
+  } else if (use_bias) {
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+      long long grow;
+      const bool valid = gemm_row_map(p, m_tile, 64 * h + 16 * wl + (lane >> 2) + 8 * t, grow);
+      // keep per-row lookups in range; the tensor map clips the rest
+      const long long boff = (valid ? grow / e.bias_group_rows : 0) * static_cast<long long>(N);
+      float2 b[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = n_base + 8 * j + 2 * q;  // N % 8 == 0: col + 1 < N iff col < N
+        const float2 v = __ldg(reinterpret_cast<const float2*>(e.bias + boff + (col < N ? col : 0)));
+        b[j] = col < N ? v : make_float2(0.f, 0.f);
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        acc[4 * j + 2 * t] = __fadd_rn(acc[4 * j + 2 * t], b[j].x);
+        acc[4 * j + 2 * t + 1] = __fadd_rn(acc[4 * j + 2 * t + 1], b[j].y);
       }
     }
-  } else {
-    // ---------------- TMA epilogues: results leave through a per-warp swizzled smem tile ----------------
-    const int lane = r & 31, quarter = r >> 5;
-    const long long grow_c = valid ? grow : 0;  // keep per-row lookups in range; the tensor map clips the rest
-    const long long bias_off = (e.bias_group_rows > 0) ? (grow_c / e.bias_group_rows) * static_cast<long long>(p.N) : 0;
-    int crd_w = 0, crd_h = 0, crd_b = 0;
-    if (p.conv) {
-      const int per_img = p.tiles_h * p.tiles_w;
-      crd_b = m_tile / per_img;
-      const int t = m_tile % per_img;
-      crd_h = (t / p.tiles_w) * kConvTH + quarter * 2;
-      crd_w = (t % p.tiles_w) * kConvTW;
-    }
-    const GemmColConst cc = gemm_col_const(e, p.N, n_base, ncols, lane);
-    const bool leader = elect_one_sync();  // issues (and owns the bulk groups of) this warp's TMA stores
-    wait_accumulator();
-    tr(1);
-    if (p.probe & 1) return;
-    int groups = store_groups;
-#pragma unroll 1
-    for (int c = 0; c < ncols / 32; ++c) {
-      const int n0 = n_base + c * 32;
-      if (n0 >= p.N) break;  // warp-uniform
-      uint32_t v[32];
+  }
+  if (e.act == ACT_GELU) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = gelu_erf(acc[i]);
+  } else if (e.act == ACT_QUICKGELU) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = quick_gelu(acc[i]);
+  } else if (e.act == ACT_RELU) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = fmaxf(acc[i], 0.f);
+  }
+}
+
+// The stores of one m64 half h: one box per 64 fp16 / 32 fp32 columns.
+template <int EPI>
+__device__ __forceinline__ void gemm_frag_store(const GemmParams& p, const float (&acc)[64], int h, int m_tile,
+                                                int n_base, int wl, int q, int rq, uint8_t* bufs, int& groups,
+                                                bool leader, GemmTrace& tr) {
+  constexpr int kBufBytes = 2048;
+  constexpr int kBoxes = (EPI == EPI_TMA_F16) ? 2 : 4;
+  constexpr int kBoxCols = kGemmBN / kBoxes;
+  constexpr int kJ = kBoxCols / 8;  // fragment column groups per box
+  const int row0 = 64 * h + 16 * wl;  // first tile row of the warp's 16
+#pragma unroll
+  for (int bx = 0; bx < kBoxes; ++bx) {
+    const int col0 = n_base + bx * kBoxCols;
+    if (col0 >= p.N) break;  // warp-uniform
+    uint8_t* buf = bufs + (groups & 1) * kBufBytes;
+    if (groups >= 2) {  // the bulk op that last used this buffer must be done READING it
+      if (leader) tma_store_wait_read<1>();
       __syncwarp();
-      gemm_acc_ld32(acc_row, c, r, v);
-      tr(2);
-      float f[32];
-      gemm_epilogue_math(e, p.N, v, grow_c, n0, bias_off, valid, f, cc, c, first_k);
-      tr(3);
-      uint8_t* buf = SINGLE_BUF ? stage_buf : stage_buf + (groups & 1) * 4096;
-      const bool first_of_group = (EPI == EPI_TMA_ADD) || ((c & 1) == 0);
-      if (first_of_group && groups >= (SINGLE_BUF ? 1 : 2)) {  // the bulk op that last used this buffer must be done READING it
-        if (leader) {
-          if (SINGLE_BUF)
-            tma_store_wait_read<0>();
-          else
-            tma_store_wait_read<1>();
-        }
-        __syncwarp();
+    }
+    uint8_t* r_lo = buf + rq * 128;  // box rows rq and rq + 8 share the swizzle phase rq
+    uint8_t* r_hi = r_lo + 8 * 128;
+#pragma unroll
+    for (int jj = 0; jj < kJ; ++jj) {
+      const int j = bx * kJ + jj;
+      if constexpr (EPI == EPI_TMA_F16) {  // columns 8 jj + 2 q, + 1: 16-byte chunk jj, bytes 4 q .. 4 q + 3
+        const int off = ((jj ^ rq) << 4) + 4 * q;
+        const __half2 lo = __floats2half2_rn(acc[4 * j], acc[4 * j + 1]);
+        const __half2 hi = __floats2half2_rn(acc[4 * j + 2], acc[4 * j + 3]);
+        *reinterpret_cast<__half2*>(r_lo + off) = lo;
+        *reinterpret_cast<__half2*>(r_hi + off) = hi;
+      } else {  // columns 8 jj + 2 q, + 1: 16-byte chunk 2 jj + q / 2, bytes 8 (q % 2) ..
+        const int off = (((2 * jj + (q >> 1)) ^ rq) << 4) + 8 * (q & 1);
+        *reinterpret_cast<float2*>(r_lo + off) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(r_hi + off) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      tr(4);
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (leader) {
       if constexpr (EPI == EPI_TMA_F16) {
-        // 32 rows x 64 fp16 columns per group: this chunk fills 16-byte slots (c&1)*4 .. +3 of the row
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          __half2 h[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(f[8 * t + 2 * i], f[8 * t + 2 * i + 1]);
-          const int slot = ((c & 1) * 4 + t) ^ (lane & 7);
-          *reinterpret_cast<uint4*>(buf + lane * 128 + slot * 16) = *reinterpret_cast<uint4*>(h);
+        if (p.conv) {  // the warp's 16 rows are pixel row 4 h + wl of the 8 x 16 conv tile
+          const int per_img = p.tiles_h * p.tiles_w;
+          const int t = m_tile % per_img;
+          tma_store_4d(&p.tma_c, buf, col0, (t % p.tiles_w) * kConvTW, (t / p.tiles_w) * kConvTH + row0 / kConvTW,
+                       m_tile / per_img);
+        } else {
+          tma_store_2d(&p.tma_c, buf, col0, m_tile * kGemmBM + row0);
         }
       } else {
-        // 32 rows x 32 fp32 columns per group
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          const int slot = t ^ (lane & 7);
-          *reinterpret_cast<float4*>(buf + lane * 128 + slot * 16) =
-              make_float4(f[4 * t], f[4 * t + 1], f[4 * t + 2], f[4 * t + 3]);
-        }
+        tma_reduce_add_2d(&p.tma_c, buf, col0, m_tile * kGemmBM + row0);
       }
-      tr(5);
-      const bool last_of_group =
-          (EPI == EPI_TMA_ADD) || ((c & 1) == 1) || (c + 1 == ncols / 32) || (n0 + 32 >= p.N);
-      if (last_of_group) {
-        fence_proxy_async_smem();
-        __syncwarp();
-        const int col0 = n_base + (c & ~1) * 32;
-        const int row0 = m_tile * kGemmBM + quarter * 32;
-        if (leader) {
-          if constexpr (EPI == EPI_TMA_F16) {
-            if (p.conv)
-              tma_store_4d(&p.tma_c, buf, col0, crd_w, crd_h, crd_b);
-            else
-              tma_store_2d(&p.tma_c, buf, col0, row0);
-          } else {
-            tma_reduce_add_2d(&p.tma_c, buf, n0, row0);
-          }
-          tma_store_commit();
-        }
-        ++groups;
-        tr(6);
-      }
+      tma_store_commit();
     }
-    store_groups = groups;
+    ++groups;
+    tr(6);
   }
+}
+
+template <int EPI>
+__device__ __forceinline__ void gemm_epilogue_frag(const GemmParams& p, float (&acc0)[64], float (&acc1)[64], int m_tile,
+                                                   int n_base, int wl, int lane, uint8_t* bufs, int& groups, bool leader,
+                                                   bool first_k, GemmTrace& tr) {
+  const GemmEpi& e = p.e;
+  const int N = p.N;
+  const bool use_bias = e.bias && first_k;
+  float2 sv[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)}, bv[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {  // independent loads, issued together
+    const int col = n_base + 64 * k + 2 * lane;
+    if (e.scale && col < N) sv[k] = __ldg(reinterpret_cast<const float2*>(e.scale + col));
+    if (use_bias && e.bias_group_rows == 0 && col < N) bv[k] = __ldg(reinterpret_cast<const float2*>(e.bias + col));
+  }
+  gemm_frag_math(p, acc0, 0, m_tile, n_base, wl, lane, sv, bv, use_bias);
+  gemm_frag_math(p, acc1, 1, m_tile, n_base, wl, lane, sv, bv, use_bias);
+  const int q = lane & 3, rq = lane >> 2;
+  gemm_frag_store<EPI>(p, acc0, 0, m_tile, n_base, wl, q, rq, bufs, groups, leader, tr);
+  gemm_frag_store<EPI>(p, acc1, 1, m_tile, n_base, wl, q, rq, bufs, groups, leader, tr);
 }
 
 // ==========================================================================================
@@ -592,7 +734,7 @@ __device__ __forceinline__ void gemm_epilogue_tile(const GemmParams& p, const fl
 //   full barrier  : per stage, armed by the producer with the stage's byte count; the TMA loads credit it
 //   empty barrier : per stage, one arrival per warp of the consumer warpgroup whose MMAs have read the stage
 //   named barriers 1 / 2 : the MMA turn of consumer warpgroup 0 / 1 (ping-pong order, see the kernel)
-//   named barriers 3 / 4 : consumer warpgroup 0 / 1 alone (its accumulator staging area)
+//   named barriers 3 / 4 : consumer warpgroup 0 / 1 alone (its accumulator staging area, staged epilogues)
 // ==========================================================================================
 template <int EPI>
 struct GemmCfg {
@@ -601,12 +743,17 @@ struct GemmCfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kEpiWarps = 8;                     // the two consumer warpgroups
   static constexpr int kThreads = 128 + 32 * kEpiWarps;   // + the producer warpgroup
-  static constexpr int kEpiBufBytes = 4096;               // one 32-row x 128 B TMA-store staging tile per warp
-  static constexpr int kStageOutBytes = (EPI == EPI_DIRECT) ? 0 : kEpiWarps * kEpiBufBytes;
-  static constexpr int kAccBytes = kGemmBM * kAccCols * 4;  // per consumer warpgroup: one staged column half
+  // staged epilogues (register-direct, and the fp16 TMA store with row sums) go through the accumulator staging areas
+  static constexpr bool kStaged = (EPI == EPI_DIRECT) || (EPI == EPI_TMA_F16_STAGED);
+  // TMA epilogues: 4 KB of TMA-store staging per warp (two 16-row boxes, gemm_epilogue_frag; one 32-row tile,
+  // gemm_tma_f16_staged)
+  static constexpr int kStageOutBytes = (EPI == EPI_DIRECT) ? 0 : kEpiWarps * 4096;
+  // staged epilogues: per consumer warpgroup, one staged column half of its tile
+  static constexpr int kAccBytes = kGemmBM * kAccCols * 4;
+  static constexpr int kAccAreaBytes = kStaged ? 2 * kAccBytes : 0;
   // operand ring | per-warp TMA-store staging (1024 B aligned) | 2 accumulator staging areas | mbarriers: <= 227 KB
-  static constexpr int kStages = (EPI == EPI_DIRECT) ? 5 : 4;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + 2 * kAccBytes + 1024 + 256;
+  static constexpr int kStages = (EPI == EPI_DIRECT) ? 5 : (EPI == EPI_TMA_F16_STAGED) ? 4 : 6;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStageOutBytes + kAccAreaBytes + 1024 + 256;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory per CTA");
   // 128 x 24 + 256 x 240 <= 65536 (= 384 x 168 at launch): what the producer warpgroup gives back, the consumers take
   // (two 64 x 128 fp32 accumulators are 128 registers per consumer thread)
@@ -662,7 +809,7 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_out = smem + Cfg::kStages * Cfg::kStageBytes;
   float* acc_stage = reinterpret_cast<float*>(stage_out + Cfg::kStageOutBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_stage) + 2 * Cfg::kAccBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_stage) + Cfg::kAccAreaBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
 
@@ -819,10 +966,12 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1)
     const int wg = (warp - 4) >> 2;
     const int wl = warp & 3;       // warp within its warpgroup: main loop fragment rows 16 wl .. 16 wl + 15 of each
     const int r = wl * 32 + lane;  // 64-row half; epilogue tile row r (thread <-> row)
-    float* acc_half = acc_stage + wg * (Cfg::kAccBytes / 4);
-    const float* acc_row = acc_half + r * kAccCols;
-    uint8_t* stage_buf = stage_out + (warp - 4) * Cfg::kEpiBufBytes;
+    float* acc_half = Cfg::kStaged ? acc_stage + wg * (Cfg::kAccBytes / 4) : nullptr;  // staged epilogues
+    const float* acc_row = Cfg::kStaged ? acc_half + r * kAccCols : nullptr;
+    uint8_t* stage_bufs = stage_out + (warp - 4) * (Cfg::kStageOutBytes / Cfg::kEpiWarps);  // TMA epilogues
     int store_groups = 0;
+    // TMA epilogues: the lane that issues (and owns the bulk groups of) this warp's TMA stores
+    const bool leader = (EPI != EPI_DIRECT) && elect_one_sync();
     int stage = 0;
     uint32_t phase = 0;
     GemmTrace tr;
@@ -884,26 +1033,34 @@ __global__ void __launch_bounds__(GemmCfg<EPI>::kThreads, 1)
         if constexpr (CLUSTER) mbar_arrive_cluster(&empty_bar[prev], rank ^ 1);
       }
       tr(12);
-      // Epilogue, one column half at a time through this warpgroup's staging area. Barrier 3 + wg: no warp of the
-      // warpgroup still reads the area (previous half or tile) when it is rewritten, and all of it is written before
-      // any warp reads it.
-      bar_sync(3 + wg, 128);
-      gemm_stage_half<0>(acc_half, acc0, wl, lane);
-      gemm_stage_half<0>(acc_half + 64 * kAccCols, acc1, wl, lane);
-      bar_sync(3 + wg, 128);
-      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES, RAGGED>(p, acc_row, n_tile * kGemmBN, kAccCols, m_tile, r, []() {},
-                                                               stage_buf, store_groups, tr, kb == 0, seg,
-                                                               gemm_ragged_k(p, img), gemm_ragged_koff(p, img));
-      bar_sync(3 + wg, 128);
-      gemm_stage_half<1>(acc_half, acc0, wl, lane);
-      gemm_stage_half<1>(acc_half + 64 * kAccCols, acc1, wl, lane);
-      bar_sync(3 + wg, 128);
-      gemm_epilogue_tile<EPI, true, GROUPED, RELU_RES, RAGGED>(p, acc_row, n_tile * kGemmBN + kAccCols, kAccCols, m_tile,
-                                                               r, []() {}, stage_buf, store_groups, tr, kb == 0, seg,
-                                                               gemm_ragged_k(p, img), gemm_ragged_koff(p, img));
+      if constexpr (Cfg::kStaged) {
+        // Epilogue, one column half at a time through this warpgroup's staging area. Barrier 3 + wg: no warp of the
+        // warpgroup still reads the area (previous half or tile) when it is rewritten, and all of it is written before
+        // any warp reads it.
+        auto epilogue_half = [&](int n_base) {
+          if constexpr (EPI == EPI_DIRECT)
+            gemm_epilogue_tile<GROUPED, RELU_RES, RAGGED>(p, acc_row, n_base, kAccCols, m_tile, r, []() {}, seg,
+                                                          gemm_ragged_k(p, img), gemm_ragged_koff(p, img));
+          else
+            gemm_tma_f16_staged(p, acc_row, n_base, kAccCols, m_tile, r, stage_bufs, store_groups, leader, tr);
+        };
+        bar_sync(3 + wg, 128);
+        gemm_stage_half<0>(acc_half, acc0, wl, lane);
+        gemm_stage_half<0>(acc_half + 64 * kAccCols, acc1, wl, lane);
+        bar_sync(3 + wg, 128);
+        epilogue_half(n_tile * kGemmBN);
+        bar_sync(3 + wg, 128);
+        gemm_stage_half<1>(acc_half, acc0, wl, lane);
+        gemm_stage_half<1>(acc_half + 64 * kAccCols, acc1, wl, lane);
+        bar_sync(3 + wg, 128);
+        epilogue_half(n_tile * kGemmBN + kAccCols);
+      } else if (!(p.probe & 1)) {
+        gemm_epilogue_frag<EPI>(p, acc0, acc1, m_tile, n_tile * kGemmBN, wl, lane, stage_bufs, store_groups, leader, kb == 0,
+                                tr);
+      }
       tr(7);
     }
-    if (EPI != EPI_DIRECT && elect_one_sync()) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem
+    if (EPI != EPI_DIRECT && leader) tma_store_wait_all();  // outstanding bulk ops read this CTA's smem
   }
   // CLUSTER: no CTA leaves while its peer may still arrive on its barriers (the peer's consumers release their last
   // stages on both CTAs)

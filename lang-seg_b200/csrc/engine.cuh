@@ -440,6 +440,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
   LSEG_CHECK_CUDA(cudaMemsetAsync(cls16, 0, sizeof(__half) * (size_t)cls_rows * D, stream));
   LSEG_ALLOC(clsb, float, (size_t)B * D);
   LSEG_ALLOC(ro, __half, BT * D);
+  plan->debug["readout3"] = ro;  // shared by the four levels: after a forward it holds the last one's
   for (int k = 0; k < 4; ++k) {
     const float* tap = taps[k];
     steps.push_back([=](const CallCtx&, cudaStream_t s) {
@@ -462,6 +463,9 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       if (add_gemm(steps, tok, D, (int)BT, (int)BT, w.readout_tok[k], e)) return -1;
     }
     LSEG_ALLOC(pk, __half, BT * c_post[k]);
+    char name[8];
+    snprintf(name, sizeof(name), "post%d", k);
+    plan->debug[name] = pk;  // [B*T, c_post[k]]
     {
       GemmEpi e = epi_none();
       e.bias = w.post_conv1x1[k].b;
@@ -664,6 +668,11 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
     LSEG_ALLOC(r, __half, px * 256);
     rn_f32[k] = f;
     rn_relu[k] = r;
+    char name[12];
+    snprintf(name, sizeof(name), "rn%d", k);
+    plan->debug[name] = f;  // NHWC fp32 [B, lh, lw, 256]
+    snprintf(name, sizeof(name), "rn%d_relu", k);
+    plan->debug[name] = r;  // its ReLU, fp16
     GemmEpi e = epi_none();
     e.out_f32 = f;
     e.out_f16_relu = r;
@@ -679,11 +688,17 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
     const long long px = static_cast<long long>(B) * h * ww;
     LSEG_ALLOC(tmp, __half, px * 256);
     LSEG_ALLOC(r2, __half, px * 256);
+    // stage buffers of this level, NHWC [B, h, ww, 256] (the _skip one at the next level's size)
+    auto name_stage = [&](const char* stage, const void* p) { plan->debug["dec" + std::to_string(k) + "_" + stage] = p; };
+    name_stage("tmp", tmp);  // shared by both units: after the forward it holds RCU2's conv1 output
+    name_stage("rcu2", r2);
     const __half* rcu2_in_relu = rn_relu[k];
     const float* rcu2_in_f32 = rn_f32[k];
     if (path_prev) {  // output = xs[0] + resConfUnit1(xs[1])
       LSEG_ALLOC(sum_f32, float, px * 256);
       LSEG_ALLOC(sum_relu, __half, px * 256);
+      name_stage("sum", sum_f32);
+      name_stage("sum_relu", sum_relu);
       // path_prev already holds xs[0] + xs[1] (previous block's output + this level's layer_rn, summed by the
       // interpolation kernel below): the residual conv adds ONE fp32 operand instead of two
       if (add_rcu(steps, w.rcu1[k], rn_relu[k], path_prev, nullptr, tmp, B, h, ww, sum_f32, nullptr, sum_relu))
@@ -718,6 +733,7 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
         e.out_f32 = t32;
       }
       if (add_gemm(steps, r2, 256, (int)px, (int)px, w.out_conv[k], e)) return -1;
+      name_stage("out_lr", low_f16 ? static_cast<const void*>(oc16) : oc32);
     }
     if (k > 0) {
       LSEG_ALLOC(pth, float, px * 4 * 256);
@@ -727,6 +743,7 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
                        : launch_upsample2x_nhwc256_f32<float>(oc32, pth, next_rn, B, h, ww, s);
       });
       path_prev = pth;
+      name_stage("skip", pth);
     } else {
       LSEG_ALLOC(pth16, __half, px * 4 * 256);
       steps.push_back([=](const CallCtx&, cudaStream_t s) {
@@ -774,6 +791,8 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
   }
   plan->featn = featn;
   plan->feat_sumsq = feat_sumsq;
+  plan->debug["featn"] = featn;
+  plan->debug["feat_sumsq"] = feat_sumsq;
   if (static_cast<int>(eng->plans.size()) >= lseg_engine::kMaxImagePlans) {
     size_t victim = 0;
     for (size_t i = 1; i < eng->plans.size(); ++i)

@@ -106,6 +106,16 @@ int lseg_debug_gemm_cluster(const lseg_gemm_args* args, int out[2]);
  * (default), 3 = pair CTAs in every plan where that is possible. Results are bit-identical in all three modes. Any other
  * value is rejected. */
 int lseg_debug_set_gemm_cluster(int mode);
+/* Debug: image plans built after this call snapshot the intermediates of trunk block `block` (ViT block, or ResNet-101
+ * bottleneck counted over all four stages) into buffers that lseg_debug_buffer names after a forward:
+ *   ViT     trace_in (fp32 stream before LN1), trace_ln1, trace_qkv, trace_attn (fp16), trace_x1 (fp32 stream after
+ *           proj), trace_ln2, trace_fc1 (fp16, after GELU), trace_out (fp32 stream after fc2);
+ *   ResNet  trace_in (fp16 block input), trace_t1, trace_t2 (fp16 conv1 / conv2 outputs), trace_id (fp32 stream before
+ *           conv3: the downsample output in a stage's first block), trace_out32 (fp32 stream after conv3), trace_out16.
+ * The snapshots are device-to-device copies, not kernel launches, and change no other buffer. -1 (the default) turns the
+ * trace off: plans then have no extra step. A block below -1 is rejected; a block at or beyond the trunk's block count
+ * makes the next forward fail before anything is launched. Cached image plans are rebuilt after a change. */
+int lseg_debug_set_trace_block(int block);
 
 /* Fused MHSA, head_dim 64 (k5; timm Attention restated at lseg_vit.py:26-39; CLIP text MHA).
  * qkv fp16 [B, N, 3*heads*64] (q|k|v thirds) -> out fp16 [B*N, heads*64].

@@ -88,7 +88,7 @@ class Weights(C.Structure):
 # every symbol include/lseg_b200.h declares (checked by tests/test_abi.py)
 SYMBOLS = [
     "lseg_last_error", "lseg_abi_version", "lseg_read_watchdog",
-    "lseg_gemm", "lseg_debug_gemm_plan", "lseg_debug_gemm_cluster", "lseg_debug_set_gemm_cluster", "lseg_mhsa", "lseg_mhsa_variant", "lseg_text_attn", "lseg_mhsa_trace", "lseg_debug_gemm_trace", "lseg_set_deterministic", "lseg_layernorm", "lseg_patchify", "lseg_pos_resize", "lseg_assemble_tokens",
+    "lseg_gemm", "lseg_debug_gemm_plan", "lseg_debug_gemm_cluster", "lseg_debug_set_gemm_cluster", "lseg_debug_set_trace_block", "lseg_mhsa", "lseg_mhsa_variant", "lseg_text_attn", "lseg_mhsa_trace", "lseg_debug_gemm_trace", "lseg_set_deterministic", "lseg_layernorm", "lseg_patchify", "lseg_pos_resize", "lseg_assemble_tokens",
     "lseg_readout_split", "lseg_im2col_3x3_s2", "lseg_stem_im2col", "lseg_maxpool3x3s2_nhwc", "lseg_subsample2_nhwc", "lseg_upsample2x_nhwc", "lseg_upsample2x_nhwc256", "lseg_l2norm_scale", "lseg_l2norm_f16",
     "lseg_upsample2x_nchw", "lseg_debug_upsample_layout", "lseg_upsample2x_nchw_bg", "lseg_upsample2x_nchw_f32", "lseg_head_block", "lseg_upsample2x_argmax", "lseg_forward_argmax", "lseg_text_embed", "lseg_text_eot_gather",
     "lseg_create", "lseg_destroy", "lseg_encode_text", "lseg_forward", "lseg_forward_lowres", "lseg_debug_buffer",
@@ -135,6 +135,7 @@ def load(build_if_missing=True):
     lib.lseg_debug_gemm_plan.argtypes = [C.POINTER(GemmArgs), C.POINTER(C.c_int * 5)]
     lib.lseg_debug_gemm_cluster.argtypes = [C.POINTER(GemmArgs), C.POINTER(C.c_int * 2)]
     lib.lseg_debug_set_gemm_cluster.argtypes = [C.c_int]
+    lib.lseg_debug_set_trace_block.argtypes = [C.c_int]
     lib.lseg_mhsa.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_mhsa_variant.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.lseg_attn_probs.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]

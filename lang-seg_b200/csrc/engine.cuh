@@ -269,6 +269,24 @@ static int add_rcu(std::vector<Step>& steps, const lseg_rcu_w& rw, const __half*
   return add_conv3x3(steps, tmp, B, h, w, 256, rw.conv2, e2);
 }
 
+// Block trace (lseg_debug_set_trace_block): a device-to-device copy of `bytes` at `src`, taken at this point of the
+// plan, into a buffer of its own that the plan's debug map names `name`.
+static int add_snapshot(ImagePlan* plan, const char* name, const void* src, size_t bytes) {
+  void* dst = plan->arena.alloc(bytes);
+  if (!dst) {
+    set_error("workspace allocation of %zu bytes failed (trace buffer %s)", bytes, name);
+    return -1;
+  }
+  plan->debug[name] = dst;
+  plan->steps.emplace_back(
+      [=](const CallCtx&, cudaStream_t s) {
+        LSEG_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+        return 0;
+      },
+      KIND_MEMSET, 0.0);
+  return 0;
+}
+
 static int get_pos_embed(lseg_engine* eng, int gh, int gw, cudaStream_t stream, const float** out) {
   auto key = std::make_pair(gh, gw);
   auto it = eng->pos_cache.find(key);
@@ -307,6 +325,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
   // ---- ViT trunk (modules/models/lseg_vit.py:166-201) ----
   LSEG_ALLOC(patch_a, __half, BT * patch_k);
   LSEG_ALLOC(patch_out, float, BT * D);
+  plan->debug["patch_out"] = patch_out;  // [B*T, D]
   LSEG_ALLOC(xbuf, float, M * D);
   LSEG_ALLOC(xn, __half, M * D);
   LSEG_ALLOC(qkv, __half, M * 3 * D);
@@ -343,7 +362,11 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
     // x += fc2(..)): that lets the GEMM epilogue use a bulk tensor reduce-add and never read x. A hooked
     // block's output (lseg_vit.py:421-426: the hook captures the block's return value) is snapshotted into
     // its tap buffer with one device-to-device copy.
+    const bool tr = i == g_trace_block;  // snapshot every intermediate of this block (lseg_debug_set_trace_block)
+    const size_t x_bytes = sizeof(float) * M * D, h_bytes = sizeof(__half) * M * D;
+    if (tr && add_snapshot(plan, "trace_in", xbuf, x_bytes)) return -1;
     add_layernorm(steps, xbuf, 0, bw.ln1_g, bw.ln1_b, xn, M, D, 1e-6f);
+    if (tr && add_snapshot(plan, "trace_ln1", xn, h_bytes)) return -1;
     {
       GemmEpi e = epi_none();
       e.bias = bw.qkv.b;
@@ -351,6 +374,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       e.ldc = 3 * D;
       if (add_gemm(steps, xn, D, (int)M, (int)M, bw.qkv, e)) return -1;
     }
+    if (tr && add_snapshot(plan, "trace_qkv", qkv, 3 * h_bytes)) return -1;
     {
       MhsaDesc md;
       md.qkv = qkv;
@@ -364,6 +388,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       steps.emplace_back([mp](const CallCtx&, cudaStream_t s) { return mhsa_run(mp, s); }, KIND_MHSA,
                          4.0 * B * heads * static_cast<double>(N) * N * 64);
     }
+    if (tr && add_snapshot(plan, "trace_attn", attn, h_bytes)) return -1;
     for (int k = 0; k < 4 && plan->attn; ++k) {  // the hook reads this block's q, k (lseg_vit.py:22-42): qkv holds them
       if (w.hooks[k] != i) continue;             // until the next block's QKV GEMM overwrites it
       AttnProbsPlan ap;
@@ -384,7 +409,9 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       e.ldc = D;
       if (add_gemm(steps, attn, D, (int)M, (int)M, bw.proj, e)) return -1;
     }
+    if (tr && add_snapshot(plan, "trace_x1", xbuf, x_bytes)) return -1;
     add_layernorm(steps, xbuf, 0, bw.ln2_g, bw.ln2_b, xn, M, D, 1e-6f);
+    if (tr && add_snapshot(plan, "trace_ln2", xn, h_bytes)) return -1;
     {
       GemmEpi e = epi_none();
       e.bias = bw.fc1.b;
@@ -393,6 +420,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       e.ldc = 4 * D;
       if (add_gemm(steps, xn, D, (int)M, (int)M, bw.fc1, e)) return -1;
     }
+    if (tr && add_snapshot(plan, "trace_fc1", hbuf, 4 * h_bytes)) return -1;
     {
       GemmEpi e = epi_none();
       e.bias = bw.fc2.b;
@@ -401,6 +429,7 @@ static int build_vit_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, int 
       e.ldc = D;
       if (add_gemm(steps, hbuf, 4 * D, (int)M, (int)M, bw.fc2, e)) return -1;
     }
+    if (tr && add_snapshot(plan, "trace_out", xbuf, x_bytes)) return -1;
     for (int k = 0; k < 4; ++k) {
       if (w.hooks[k] != i) continue;
       float* tap = taps[k];
@@ -525,6 +554,7 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
   const long long R0 = static_cast<long long>(B) * Hs * Ws;
   LSEG_ALLOC(stem_a, __half, R0 * kStemK);
   LSEG_ALLOC(stem_o, __half, R0 * 64);
+  plan->debug["stem"] = stem_o;  // NHWC fp16 [B, H/2, W/2, 64]
   steps.push_back([=](const CallCtx& c, cudaStream_t s) { return launch_stem_im2col(c.x, stem_a, B, H, W, s); });
   {
     GemmEpi e = epi_none();
@@ -537,6 +567,7 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
   }
   int h = Hs / 2, ww = Ws / 2;  // after the 3x3 stride-2 max pool
   LSEG_ALLOC(pool_o, __half, static_cast<long long>(B) * h * ww * 64);
+  plan->debug["pool"] = pool_o;  // NHWC fp16 [B, H/4, W/4, 64]
   steps.push_back([=](const CallCtx&, cudaStream_t s) { return launch_maxpool3x3s2_nhwc(stem_o, pool_o, B, Hs, Ws, 64, s); });
   const __half* x16 = pool_o;
   int cin = 64, blk = 0;
@@ -565,6 +596,8 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
       }
       const int hi = (i == 0) ? h : ho, wi = (i == 0) ? ww : wo;
       const long long pxi = static_cast<long long>(B) * hi * wi;
+      const bool tr = blk == g_trace_block;  // snapshot every intermediate of this block (lseg_debug_set_trace_block)
+      if (tr && add_snapshot(plan, "trace_in", x16, sizeof(__half) * pxi * cin)) return -1;
       {  // conv1 1x1 + bn1 + relu
         GemmEpi e = epi_none();
         e.scale = bw.bn1_scale;
@@ -574,6 +607,7 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
         e.ldc = width;
         if (add_gemm(steps, x16, cin, (int)pxi, (int)pxi, bw.conv1, e)) return -1;
       }
+      if (tr && add_snapshot(plan, "trace_t1", t1, sizeof(__half) * pxi * width)) return -1;
       {  // conv2 3x3 (stride here, torchvision v1.5) + bn2 + relu
         GemmEpi e = epi_none();
         e.scale = bw.bn2_scale;
@@ -589,6 +623,7 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
           if (add_gemm(steps, a2, 9 * width, (int)px, (int)px, bw.conv2, e)) return -1;
         }
       }
+      if (tr && add_snapshot(plan, "trace_t2", t2, sizeof(__half) * px * width)) return -1;
       if (i == 0) {  // identity = bn_d(conv_d 1x1 stride s (x)) -> the stage's fp32 stream
         const __half* xs = x16;
         if (stride == 2) {
@@ -604,6 +639,7 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
         e.ldc = cout;
         if (add_gemm(steps, xs, cin, (int)px, (int)px, bw.down, e)) return -1;
       }
+      if (tr && add_snapshot(plan, "trace_id", y32, sizeof(float) * px * cout)) return -1;
       __half* y16 = (i & 1) ? y16b : y16a;
       {  // conv3 1x1 + bn3, + identity, relu -> fp32 stream (in place) and its fp16 copy
         GemmEpi e = epi_none();
@@ -616,6 +652,9 @@ static int build_resnet_trunk(lseg_engine* eng, ImagePlan* plan, int B, int H, i
         e.ldc = cout;
         if (add_gemm(steps, t2, width, (int)px, (int)px, bw.conv3, e)) return -1;
       }
+      if (tr && (add_snapshot(plan, "trace_out32", y32, sizeof(float) * px * cout) ||
+                 add_snapshot(plan, "trace_out16", y16, sizeof(__half) * px * cout)))
+        return -1;
       x16 = y16;
       cin = cout;
     }
@@ -648,6 +687,12 @@ static int build_image_plan(lseg_engine* eng, int B, int H, int W, bool attn, cu
   std::vector<Step>& steps = plan->steps;
   __half* layer_in[4];  // NHWC fp16 inputs of scratch.layerN_rn
   int c_post[4], lh[4], lw[4];
+  const int blocks = w.trunk == 1 ? w.rn_layers[0] + w.rn_layers[1] + w.rn_layers[2] + w.rn_layers[3] : w.vit_depth;
+  if (g_trace_block >= blocks) {  // before anything is allocated or launched
+    set_error("lseg_debug_set_trace_block: trace block %d is not a block of this trunk, which has %d blocks",
+              g_trace_block, blocks);
+    return -1;
+  }
   if (w.trunk == 1) {
     if (build_resnet_trunk(eng, plan.get(), B, H, W, stream, layer_in, c_post, lh, lw)) return -1;
   } else {

@@ -48,6 +48,7 @@ static unsigned long long* g_gemm_trace = nullptr;  // debug (lseg_debug_gemm_tr
 static int g_gemm_probe = 0;
 static int g_mhsa_variant = 0;   // kernel the engine's ViT attention runs (lseg_mhsa_variant documents the numbering)
 static int g_gemm_cluster_mode = 2;  // lseg_debug_set_gemm_cluster: 1 never, 2 the planner's rule, 3 wherever allowed
+static int g_trace_block = -1;       // lseg_debug_set_trace_block: trunk block whose intermediates image plans snapshot
 // Which gemm_tc_kernel instantiation runs a plan (numbering of lseg_debug_gemm_plan's out[4]).
 enum GemmKernel { GK_DIRECT = 0, GK_TMA_F16 = 1, GK_TMA_ADD = 2, GK_FIXED_SPLIT = 3, GK_GROUPED_NCHW = 4, GK_RELU_RES = 5,
                   GK_RAGGED = 6, GK_COUNT = 7 };
@@ -1046,6 +1047,16 @@ int lseg_debug_set_gemm_cluster(int mode) {
   if (ensure_init()) return -1;
   if (mode != g_gemm_cluster_mode) ++g_plan_epoch;
   g_gemm_cluster_mode = mode;
+  return 0;
+}
+
+int lseg_debug_set_trace_block(int block) {
+  if (block < -1) {
+    set_error("debug_set_trace_block: block must be -1 (off) or a trunk block index, got %d", block);
+    return -1;
+  }
+  if (block != g_trace_block) ++g_plan_epoch;
+  g_trace_block = block;
   return 0;
 }
 

@@ -129,6 +129,12 @@ def set_gemm_cluster(mode):
     check(load().lseg_debug_set_gemm_cluster(int(mode)))
 
 
+def set_trace_block(block):
+    """Snapshot the intermediates of trunk block `block` in later image plans (lseg_debug_set_trace_block: trace_* debug
+    buffers after a forward); -1 turns the trace off (the default)."""
+    check(load().lseg_debug_set_trace_block(int(block)))
+
+
 def _attn_out(out, rows, heads, device, what):
     """A caller-given output must be fp16 [rows, heads*64]: the kernel writes exactly that much, unchecked."""
     if out is None:

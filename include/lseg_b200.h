@@ -31,7 +31,9 @@ int lseg_abi_version(void);
 /* Reads and clears the device-side barrier watchdog: out[0] != 0 means a kernel timed out on an
  * mbarrier (out[0] = wait tag, out[1] = block, out[2] = thread, out[3] = parity). Synchronises stream.
  * When no barrier timed out it reports instead the first image whose metric group id was outside [0, G) since the last
- * read (section "segmentation metrics"): out[0] = 78, out[1] = image, out[2] = its group id, out[3] = G. */
+ * read (section "segmentation metrics"): out[0] = 78, out[1] = image, out[2] = its group id, out[3] = G. When neither is
+ * pending, the first loss target outside [0, K) other than ignore_index (section "cross-entropy"): out[0] = 79,
+ * out[1] = image, out[2] = pixel index y * W + x, out[3] = the target value (both clamped to int). */
 int lseg_read_watchdog(int out[4], void* stream);
 
 /* ---- stage ops (each one is parity-tested on its own; SURVEY.md section 2b numbering) ------------ */
@@ -286,6 +288,24 @@ int lseg_seg_stats_scores(const float* scores, const long long* target, const in
 int lseg_seg_stats_mask(const long long* pred, const long long* target, const int* group, int B, int H, int W, int nclass,
                         int G, long long* stats, void* stream);
 
+/* ---- cross-entropy ----------------------------------------------------------------------------------------------------
+ * The validation loss of LSegmentationModule.validation_step (modules/lsegmentation_module.py:86-105): PyTorch-Encoding's
+ * SegmentationLosses with se_loss = aux = False and no class weight, i.e. CrossEntropyLoss(ignore_index) with mean
+ * reduction. Per pixel with target t and fp32 logits v_0 .. v_{K-1}:
+ *     t == ignore_index : skipped
+ *     t outside [0, K)  : loss NaN, counted; the first such pixel is recorded (lseg_read_watchdog tag 79: image, pixel
+ *                         index y * W + x, target value) instead of torch's device-side assert
+ *     otherwise         : loss = (m + log s) - v_t, m = max_k v_k, s = sum_k exp(v_k - m) (online, classes in order)
+ * in fp32 (expf / logf); a NaN logit gives a NaN loss. The calls ADD {sum of losses, counted pixels} to loss double[2]
+ * (8-byte aligned) and never clear it: the mean is loss[0] / loss[1] (NaN when every pixel is ignored). Each block sums
+ * its pixels in fp64 in a fixed order into a slot of `partials` and one further launch adds the slots in index order,
+ * without floating-point atomics: the same call gives the same bits every time.
+ * lseg_xent_scores: scores fp32 [B,K,H,W] (any H, W), target int64 [B,H,W]; partials_len >= 2 * B * ceil(H*W / 1024)
+ * doubles. Rejected by name before any launch: NULL or misaligned pointers, B outside [1, 65535], K <= 0, H or W <= 0,
+ * partials too short. */
+int lseg_xent_scores(const float* scores, const long long* target, long long ignore_index, int B, int K, int H, int W,
+                     double* loss, double* partials, long long partials_len, void* stream);
+
 /* ---- peer memory: the logits gather (SURVEY.md section 8(e)), one process per GPU over NVLink 5 / NVSwitch ----------
  * Replaces the thread-per-GPU DataParallel gather of additional_utils/models.py:35-53. A rank allocates a buffer its peers
  * can map (CUDA IPC; the 64-byte handle travels through any host channel, e.g. torch.distributed.all_gather_object);
@@ -437,6 +457,18 @@ int lseg_forward_segstats(lseg_engine* e, const float* x, int B, int H, int W, c
                           long long text_image_stride, const long long* target, const int* group, int nclass, int G,
                           long long* stats, long long* mask, float* logits, void* stream);
 
+/* lseg_forward_segstats with the validation cross-entropy fused into the same output kernel (section "cross-entropy"):
+ * adds {sum of per-pixel losses, counted pixels} of the logits lseg_forward returns against loss_target int64 [B,H,W]
+ * to loss double[2]. loss_target NULL means the metric target. The metric (target, group, nclass, G, stats as in
+ * lseg_forward_segstats) is optional here: target, group and stats all NULL, or target and stats given. mask and logits
+ * are optional outputs with the bits lseg_forward_argmax / lseg_forward write. partials: caller workspace of
+ * partials_len >= 2 * B * ceil(H / 8) doubles, 8-byte aligned. Needs W <= 1024 besides lseg_forward's rules; every
+ * argument is checked, and rejected by name, before the first launch. */
+int lseg_forward_xent(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
+                      long long text_image_stride, const long long* target, const int* group, int nclass, int G,
+                      long long* stats, const long long* loss_target, long long ignore_index, double* loss,
+                      double* partials, long long partials_len, long long* mask, float* logits, void* stream);
+
 /* Same as lseg_forward, but brackets every kernel launch with CUDA events on `stream`, synchronises,
  * and returns per-launch device time (ms), kernel class (0 elementwise, 1 wgmma GEMM, 2 MHSA,
  * 3 LayerNorm) and ALGORITHMIC flops of the launch. Used by bench.py for the roofline block. */
@@ -491,6 +523,15 @@ int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, i
                float* logits, long long* mask,
                const long long* target, const int* group, int nclass, int G, long long* stats,
                void* stream);
+
+/* lseg_query with the cross-entropy of lseg_forward_xent: same loss arguments and rules, same result bit for bit as
+ * lseg_forward_xent on the image that produced `emb`. */
+int lseg_query_xent(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W,
+                    const void* text, int K, long long text_image_stride,
+                    float* logits, long long* mask,
+                    const long long* target, const int* group, int nclass, int G, long long* stats,
+                    const long long* loss_target, long long ignore_index, double* loss, double* partials,
+                    long long partials_len, void* stream);
 
 /* Ragged batch: every image brings its own label set (open-vocabulary serving: one prompt per request, batched for
  * throughput). Image b's k[b] labels are rows text_row[b] .. text_row[b] + k[b] - 1 of ONE packed text operand `text`

@@ -100,6 +100,7 @@ SYMBOLS = [
     "lseg_encode_image", "lseg_query", "lseg_embedding_features",
     "lseg_forward_ragged", "lseg_query_ragged", "lseg_gemm_ragged",
     "lseg_attn_probs", "lseg_encode_image_attention",
+    "lseg_xent_scores", "lseg_forward_xent", "lseg_query_xent",
 ]
 
 _lib = None
@@ -201,6 +202,15 @@ def load(build_if_missing=True):
     lib.lseg_forward_segstats.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                           C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p]
+    _xent = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong]  # loss_target .. partials_len
+    lib.lseg_xent_scores.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]
+    lib.lseg_forward_xent.argtypes = ([C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                       C.c_longlong, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p] + _xent +
+                                      [C.c_void_p, C.c_void_p, C.c_void_p])
+    lib.lseg_query_xent.argtypes = ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                     C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                     C.c_void_p] + _xent + [C.c_void_p])
     lib.lseg_encode_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_void_p]
     lib.lseg_encode_image_attention.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblseg_b200.so")
 SOURCES = ["lseg_b200.cu"]
-HEADERS = ["common.cuh", "gemm_tc.cuh", "mhsa.cuh", "attn_probs.cuh", "text_attn.cuh", "p2p.cuh", "evaluator.cuh", "segstats.cuh", "elementwise.cuh", "embed.cuh", "engine.cuh"]
+HEADERS = ["common.cuh", "gemm_tc.cuh", "mhsa.cuh", "attn_probs.cuh", "text_attn.cuh", "p2p.cuh", "evaluator.cuh", "segstats.cuh", "xent.cuh", "elementwise.cuh", "embed.cuh", "engine.cuh"]
 
 
 def nvcc_path():

@@ -16,6 +16,7 @@ namespace lseg {
 }  // namespace lseg
 
 #include "segstats.cuh"
+#include "xent.cuh"
 
 namespace lseg {
 
@@ -805,13 +806,19 @@ static inline int launch_upsample2x_nchw_bg(const __half* x, float* y, long long
 // and counts them into the block's histogram (all 8 warps of a block belong to one image, hence one counter row), which
 // is flushed once per block; the mask store becomes optional (mask may be nullptr).
 // ------------------------------------------------------------------------------------------
+// kLoss (upsample2x_xent_kernel, always with kStats) adds the cross-entropy of xent.cuh: each lane reads its pixels'
+// loss targets before the class loop, runs the online log-sum-exp beside the running maximum (which is its m) and picks
+// the target class's value on the way; after the loop it adds the pixels' losses to its fp64 running sum.
 constexpr int kArgJ = 16;  // outputs per lane per pass (Wo <= 512 in one pass)
+constexpr int kXentArgJ = 8;  // the same for the loss variant: 128 registers, two blocks per SM (16: 247, one)
 // plane0: index of the image's first low-res plane in lr (b * K for one label set; its K planes follow it)
-template <typename TIn, bool kStats>
+template <typename TIn, bool kStats, bool kLoss = false, int J = kArgJ>
 __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr, long long* __restrict__ mask, int K, int H,
                                                       int W, int b, int oy, int lane, float (*line)[kUpMaxW],
                                                       const SegStatsArgs& st, int* hist, unsigned long long* grow,
-                                                      int& labeled, int& correct, long long plane0) {
+                                                      int& labeled, int& correct, long long plane0,
+                                                      const XentArgs* xe = nullptr, double* lsum = nullptr,
+                                                      int* lcount = nullptr) {
   const int Ho = 2 * H, Wo = 2 * W;
   const float sh = (Ho > 1) ? static_cast<float>(H - 1) / (Ho - 1) : 0.f;
   const float sw = (Wo > 1) ? static_cast<float>(W - 1) / (Wo - 1) : 0.f;
@@ -822,12 +829,12 @@ __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr
   const long long plane_sz = static_cast<long long>(H) * W;
   const TIn* img = lr + plane0 * plane_sz;
   const long long row_off = (static_cast<long long>(b) * Ho + oy) * Wo;
-  for (int ox0 = 0; ox0 < Wo; ox0 += 32 * kArgJ) {
-    int xa[kArgJ], xb[kArgJ];
-    float lx[kArgJ], best[kArgJ];
-    int arg[kArgJ];
+  for (int ox0 = 0; ox0 < Wo; ox0 += 32 * J) {
+    int xa[J], xb[J];
+    float lx[J], best[J];
+    int arg[J];
 #pragma unroll
-    for (int j = 0; j < kArgJ; ++j) {
+    for (int j = 0; j < J; ++j) {
       const int ox = min(ox0 + lane + 32 * j, Wo - 1);
       const float fx = sw * ox;
       const int xi = static_cast<int>(fx);
@@ -836,6 +843,18 @@ __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr
       xb[j] = min(xa[j] + 1, W - 1);
       best[j] = -INFINITY;
       arg[j] = 0;
+    }
+    float ls[kLoss ? J : 1], lv[kLoss ? J : 1];
+    int lt[kLoss ? J : 1];
+    if constexpr (kLoss) {
+      const long long* trow = xe->target + row_off;
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int ox = ox0 + lane + 32 * j;
+        lt[j] = ox < Wo ? xent_class(__ldg(trow + ox), *xe, K, b, static_cast<long long>(oy) * Wo + ox) : -1;
+        ls[j] = 0.f;
+        lv[j] = 0.f;
+      }
     }
     for (int k = 0; k < K; ++k) {
       const TIn* r0 = img + k * plane_sz + static_cast<long long>(y0) * W;
@@ -852,8 +871,12 @@ __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr
       }
       __syncwarp();  // line k visible; line k-1 (other buffer) is free again after this point for iteration k+1
 #pragma unroll
-      for (int j = 0; j < kArgJ; ++j) {
+      for (int j = 0; j < J; ++j) {
         const float val = lerp2(1.f - lx[j], v[xa[j]], lx[j], v[xb[j]]);
+        if constexpr (kLoss) {
+          xent_lse_step(val, best[j], ls[j]);
+          if (k == lt[j]) lv[j] = val;
+        }
         if (val > best[j]) {  // strict: the first maximal class wins, like torch.max on the logits
           best[j] = val;
           arg[j] = k;
@@ -861,23 +884,27 @@ __device__ __forceinline__ void upsample2x_argmax_row(const TIn* __restrict__ lr
       }
     }
     __syncwarp();
+    if constexpr (kLoss) {
+#pragma unroll
+      for (int j = 0; j < J; ++j) xent_add_pixel(lt[j], best[j], ls[j], lv[j], *lsum, *lcount);
+    }
     if constexpr (kStats) {
       if (grow) {  // nullptr: the image's group id is out of range
         const long long* trow = st.target + row_off;
-        long long t[kArgJ];
+        long long t[J];
 #pragma unroll
-        for (int j = 0; j < kArgJ; ++j) {
+        for (int j = 0; j < J; ++j) {
           const int ox = ox0 + lane + 32 * j;
           t[j] = ox < Wo ? __ldg(trow + ox) : -1;
         }
 #pragma unroll
-        for (int j = 0; j < kArgJ; ++j) seg_count_pixel(arg[j], t[j], st.nclass, hist, grow, labeled, correct);
+        for (int j = 0; j < J; ++j) seg_count_pixel(arg[j], t[j], st.nclass, hist, grow, labeled, correct);
       }
       if (!mask) continue;
     }
     long long* orow = mask + row_off;
 #pragma unroll
-    for (int j = 0; j < kArgJ; ++j) {
+    for (int j = 0; j < J; ++j) {
       const int ox = ox0 + lane + 32 * j;
       if (ox < Wo) orow[ox] = arg[j];
     }
@@ -967,6 +994,45 @@ static inline int launch_upsample2x_segstats(const TIn* lr, long long* mask, int
   launch_pdl(upsample2x_argmax_kernel<TIn, true>, dim3((2 * H + 7) / 8, B), dim3(256), seg_smem_bytes(st.nclass), s, lr,
              mask, K, H, W, st);
   LSEG_LAUNCH_CHECK();
+}
+
+// The same output stage with the cross-entropy of `xe` (xent.cuh), the metric counters of `st` when st.stats is non-NULL,
+// and the mask when `mask` is non-NULL. Each block writes one (loss sum, count) partial; xent_finish_kernel adds them.
+template <typename TIn>
+__global__ void __launch_bounds__(256) upsample2x_xent_kernel(const TIn* __restrict__ lr, long long* __restrict__ mask,
+                                                              int K, int H, int W, SegStatsArgs st, XentArgs xe) {
+  griddep_launch_dependents();
+  griddep_wait();
+  __shared__ __align__(16) float line[8][2][kUpMaxW];
+  extern __shared__ int seg_hist[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.y;
+  const int oy = blockIdx.x * 8 + warp;
+  unsigned long long* grow = nullptr;
+  int* hist = nullptr;
+  if (st.stats) {
+    const int g = seg_group_row(st, b, blockIdx.x == 0 && threadIdx.x == 0);
+    grow = g < 0 ? nullptr : reinterpret_cast<unsigned long long*>(st.stats + static_cast<long long>(g) * (3 * st.nclass + 2));
+    hist = grow && st.nclass <= kSegSmemMaxClass ? seg_hist : nullptr;
+    seg_block_begin(hist, st.nclass);
+  }
+  int labeled = 0, correct = 0, lcount = 0;
+  double lsum = 0.0;
+  if (oy < 2 * H)  // warps past the last row still take part in the block's reductions
+    upsample2x_argmax_row<TIn, true, true, kXentArgJ>(lr, mask, K, H, W, b, oy, lane, line[warp], st, hist, grow, labeled,
+                                                      correct, static_cast<long long>(b) * K, &xe, &lsum, &lcount);
+  if (grow) seg_block_finish(hist, grow, st.nclass, labeled, correct);
+  xent_block_store(lsum, static_cast<double>(lcount), reinterpret_cast<double*>(&line[0][0][0]), xe.partials,
+                   static_cast<long long>(b) * gridDim.x + blockIdx.x);
+}
+template <typename TIn>
+static inline int launch_upsample2x_xent(const TIn* lr, long long* mask, int B, int K, int H, int W, const SegStatsArgs& st,
+                                         const XentArgs& xe, cudaStream_t s) {
+  if (check_upsample2x_argmax(B, K, H, W)) return -1;
+  launch_pdl(upsample2x_xent_kernel<TIn>, dim3((2 * H + 7) / 8, B), dim3(256), st.stats ? seg_smem_bytes(st.nclass) : 0, s,
+             lr, mask, K, H, W, st, xe);
+  LSEG_CHECK_CUDA(cudaGetLastError());
+  return launch_xent_finish(xe, static_cast<long long>((2 * H + 7) / 8) * B, s);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -27,6 +27,7 @@ struct CallCtx {
                          // fp16 matmul, lseg_net.py:194-196) instead of the plan's own buffer; may be PEER memory — the
                          // pixel x text GEMM then stores straight into another GPU's gather buffer over NVLink
   const SegStatsArgs* seg = nullptr;  // optional metric counters, fused with the argmax output stage (out_mask optional)
+  const XentArgs* xent = nullptr;     // optional cross-entropy, fused with the same stage (seg and out_mask optional)
   // ragged batch (lseg_forward_ragged / lseg_query_ragged): image b's rag_k[b] labels are rows rag_text_row[b] .. of
   // `text` (rag_text_rows readable rows); K is then the sum of rag_k, and the logits / low-res planes are packed by image
   const int* rag_k = nullptr;
@@ -1144,7 +1145,14 @@ static int run_tail(lseg_engine* eng, const CallCtx& ctx, int B, int H, int W, c
     if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
   }
   // ---- fused output_conv + torch.max(.., 1)[1] (SURVEY.md 8(f) row 2): the fp32 logits are never materialised ----
-  if (ctx.seg) {  // ... and counted into the metric rows in the same kernel
+  if (ctx.xent) {  // ... with the loss (and the metric counters when ctx.seg is set) in the same kernel
+    const SegStatsArgs st = ctx.seg ? *ctx.seg : SegStatsArgs{};
+    if (lr32 ? launch_upsample2x_xent(lr32, ctx.out_mask, B, ctx.K, h2, w2, st, *ctx.xent, stream)
+             : launch_upsample2x_xent(lr, ctx.out_mask, B, ctx.K, h2, w2, st, *ctx.xent, stream))
+      return -1;
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;  // the loss kernel and its one-block finish
+    if (note_launch(prof, launches, KIND_EW, 0.0, stream)) return -1;
+  } else if (ctx.seg) {  // ... and counted into the metric rows in the same kernel
     if (lr32 ? launch_upsample2x_segstats(lr32, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream)
              : launch_upsample2x_segstats(lr, ctx.out_mask, B, ctx.K, h2, w2, *ctx.seg, stream))
       return -1;
@@ -1492,6 +1500,53 @@ int lseg_forward_segstats(lseg_engine* e, const float* x, int B, int H, int W, c
   return run_forward(e, ctx, B, H, W, static_cast<cudaStream_t>(stream));
 }
 
+// The rules the fused loss adds to a forward / query: the metric arguments (all NULL, or target and stats given), the loss
+// target (NULL: the metric target), accumulator and partials, and W <= 1024. Fills st / xe on success.
+static int check_fused_xent(const char* fn, const void* input, int B, int H, int W, const long long* target, const int* group,
+                            int nclass, int G, long long* stats, const long long* loss_target, long long ignore_index,
+                            double* loss, double* partials, long long partials_len, lseg::SegStatsArgs* st,
+                            lseg::XentArgs* xe) {
+  using namespace lseg;
+  *st = SegStatsArgs{target, group, stats, nclass, G};
+  if ((target || group || stats) && seg_stats_check(fn, input, *st, B, H, W)) return -1;
+  *xe = XentArgs{loss_target ? loss_target : target, ignore_index, partials, loss};
+  if (B <= 0 || B > 65535) return set_error("%s: B=%d must be in [1, 65535]", fn, B), -1;
+  if (H <= 0 || W <= 0) return set_error("%s: H=%d, W=%d must be positive", fn, H, W), -1;
+  if (xent_check(fn, *xe, partials_len, xent_partials_fused(B, H))) return -1;
+  if (W > 2 * kUpMaxW) return set_error("%s: W=%d must be <= %d with the loss", fn, W, 2 * kUpMaxW), -1;
+  return 0;
+}
+
+int lseg_forward_xent(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
+                      long long text_image_stride, const long long* target, const int* group, int nclass, int G,
+                      long long* stats, const long long* loss_target, long long ignore_index, double* loss,
+                      double* partials, long long partials_len, long long* mask, float* logits, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_forward_xent";
+  // every rule is checked here, before the forward enqueues its first kernel
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!x) return set_error("%s: null x", fn), -1;
+  if (!text) return set_error("%s: null text", fn), -1;
+  if (K <= 0) return set_error("%s: K=%d labels must be positive", fn, K), -1;
+  SegStatsArgs st;
+  XentArgs xe;
+  if (check_fused_xent(fn, x, B, H, W, target, group, nclass, G, stats, loss_target, ignore_index, loss, partials,
+                       partials_len, &st, &xe))
+    return -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  CallCtx ctx;
+  ctx.x = x;
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = K;
+  ctx.text_image_stride = text_image_stride;
+  ctx.out = logits;     // optional
+  ctx.out_mask = mask;  // optional
+  ctx.out_lr = nullptr;
+  ctx.seg = stats ? &st : nullptr;
+  ctx.xent = &xe;
+  return run_forward(e, ctx, B, H, W, static_cast<cudaStream_t>(stream));
+}
+
 int lseg_forward_profiled(lseg_engine* e, const float* x, int B, int H, int W, const void* text, int K,
                           long long text_image_stride, float* out, void* stream, float* step_ms, int* step_kind,
                           double* step_flops, int cap, int* count) {
@@ -1629,6 +1684,52 @@ int lseg_query(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, i
   ctx.out = logits;
   ctx.out_mask = mask;
   ctx.seg = seg ? &st : nullptr;
+  int launches = 0;
+  __half* lr = nullptr;
+  if (run_tail(e, ctx, B, H, W, static_cast<const __half*>(emb), emb_sumsq, static_cast<cudaStream_t>(stream), nullptr,
+               &launches, &lr))
+    return -1;
+  e->last_launches = launches;
+  return 0;
+}
+
+int lseg_query_xent(lseg_engine* e, const void* emb, const float* emb_sumsq, int B, int H, int W, const void* text, int K,
+                    long long text_image_stride, float* logits, long long* mask, const long long* target,
+                    const int* group, int nclass, int G, long long* stats, const long long* loss_target,
+                    long long ignore_index, double* loss, double* partials, long long partials_len, void* stream) {
+  using namespace lseg;
+  const char* fn = "lseg_query_xent";
+  // every rule is checked here, before the first launch
+  if (!e) return set_error("%s: null engine", fn), -1;
+  if (!emb) return set_error("%s: null emb", fn), -1;
+  if (!emb_sumsq) return set_error("%s: null emb_sumsq", fn), -1;
+  if (!text) return set_error("%s: null text", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb) % 16) return set_error("%s: emb must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(emb_sumsq) % 16) return set_error("%s: emb_sumsq must be 16-byte aligned", fn), -1;
+  if (reinterpret_cast<uintptr_t>(text) % 16) return set_error("%s: text must be 16-byte aligned", fn), -1;
+  if (logits && reinterpret_cast<uintptr_t>(logits) % 16) return set_error("%s: logits must be 16-byte aligned", fn), -1;
+  if (mask && reinterpret_cast<uintptr_t>(mask) % 8) return set_error("%s: mask must be 8-byte aligned", fn), -1;
+  if (K <= 0) return set_error("%s: K=%d labels must be positive", fn, K), -1;
+  if (text_image_stride < 0 || (text_image_stride > 0 && text_image_stride < K))
+    return set_error("%s: text_image_stride=%lld must be 0 or >= K=%d", fn, text_image_stride, K), -1;
+  SegStatsArgs st;
+  XentArgs xe;
+  if (check_fused_xent(fn, emb, B, H, W, target, group, nclass, G, stats, loss_target, ignore_index, loss, partials,
+                       partials_len, &st, &xe))
+    return -1;
+  if (check_image_shape(fn, B, H, W)) return -1;
+  if (ensure_init()) return -1;
+  LSEG_CHECK_CUDA(cudaSetDevice(e->device));
+  if (ensure_init()) return -1;
+  CallCtx ctx;
+  memset(&ctx, 0, sizeof(ctx));
+  ctx.text = static_cast<const __half*>(text);
+  ctx.K = K;
+  ctx.text_image_stride = text_image_stride;
+  ctx.out = logits;
+  ctx.out_mask = mask;
+  ctx.seg = stats ? &st : nullptr;
+  ctx.xent = &xe;
   int launches = 0;
   __half* lr = nullptr;
   if (run_tail(e, ctx, B, H, W, static_cast<const __half*>(emb), emb_sumsq, static_cast<cudaStream_t>(stream), nullptr,

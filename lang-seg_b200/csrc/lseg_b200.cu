@@ -205,7 +205,8 @@ static int make_tmap(CUtensorMap* out, CUtensorMapDataType dtype, const void* ba
 }
 
 // A barrier timeout (g_watchdog) is reported first; a bad metric group id (g_segstats_error, tag kSegStatsTag) when no
-// timeout is pending. Only the reported record is cleared, so a second call returns the other one.
+// timeout is pending; a bad loss target (g_xent_error, tag kXentTag) when neither is. Only the reported record is
+// cleared, so further calls return the others.
 int read_watchdog(int out[4], cudaStream_t stream) {
   LSEG_CHECK_CUDA(cudaStreamSynchronize(stream));
   LSEG_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_watchdog, sizeof(int) * 4));
@@ -215,7 +216,12 @@ int read_watchdog(int out[4], cudaStream_t stream) {
     return 0;
   }
   LSEG_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_segstats_error, sizeof(int) * 4));
-  if (out[0] != 0) LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_segstats_error, zero, sizeof(zero)));
+  if (out[0] != 0) {
+    LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_segstats_error, zero, sizeof(zero)));
+    return 0;
+  }
+  LSEG_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_xent_error, sizeof(int) * 4));
+  if (out[0] != 0) LSEG_CHECK_CUDA(cudaMemcpyToSymbol(g_xent_error, zero, sizeof(zero)));
   return 0;
 }
 
@@ -1313,6 +1319,13 @@ int lseg_seg_stats_mask(const long long* pred, const long long* target, const in
   if (ensure_init()) return -1;
   return launch_seg_stats_mask(pred, B, H, W, SegStatsArgs{target, group, stats, nclass, G},
                                static_cast<cudaStream_t>(stream));
+}
+
+int lseg_xent_scores(const float* scores, const long long* target, long long ignore_index, int B, int K, int H, int W,
+                     double* loss, double* partials, long long partials_len, void* stream) {
+  if (ensure_init()) return -1;
+  return launch_xent_scores(scores, B, K, H, W, XentArgs{target, ignore_index, partials, loss}, partials_len,
+                            static_cast<cudaStream_t>(stream));
 }
 
 int lseg_text_embed(const int64_t* tokens, const float* tok_emb, const float* pos_emb, void* x, int K, int L, int Wd,

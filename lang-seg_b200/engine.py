@@ -185,6 +185,70 @@ class Engine:
                                                       C.c_void_p(stats.data_ptr()), mp, lp, _stream()))
         return stats
 
+    def _loss_args(self, b, h, w, k, loss_target, acc, ignore_index, target, stats, nclass, group, mask, logits):
+        """ctypes arguments of lseg_forward_xent / lseg_query_xent from `target` to `partials_len`, after checking the
+        tensors; the partials workspace comes back too, so that it outlives the call's enqueue."""
+        from .ops import _check_stats, _group_ptr, xent_partials
+        if loss_target.device != self.device or loss_target.dtype != torch.int64 or tuple(loss_target.shape) != (b, h, w):
+            raise ValueError(f"loss target must be int64 [B,H,W] = {(b, h, w)} on {self.device}")
+        if acc.device != self.device or acc.dtype != torch.float64 or acc.numel() != 2 or not acc.is_contiguous():
+            raise ValueError(f"acc must be a contiguous float64 tensor of 2 elements on {self.device}")
+        for name, t, dt, shape in (("mask", mask, torch.int64, (b, h, w)), ("logits", logits, torch.float32, (b, k, h, w))):
+            if t is not None and (t.device != self.device or t.dtype != dt or tuple(t.shape) != shape or
+                                  not t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous {dt} {shape} tensor on {self.device}")
+        tp = gp = sp = g = None
+        if stats is not None or target is not None:
+            if stats is None or target is None:
+                raise ValueError("target and stats go together")
+            _check_stats(stats, nclass)
+            if target.device != self.device or target.dtype != torch.int64 or tuple(target.shape) != (b, h, w):
+                raise ValueError(f"target must be int64 [B,H,W] = {(b, h, w)} on {self.device}")
+            if stats.device != self.device or not stats.is_contiguous():
+                raise ValueError(f"stats must be a contiguous tensor on {self.device}")
+            target = target.contiguous()
+            g, gp = _group_ptr(group, stats, b)
+            tp, sp = C.c_void_p(target.data_ptr()), C.c_void_p(stats.data_ptr())
+        loss_target = loss_target.contiguous()
+        part = torch.empty((xent_partials(b, h, w, True), 2), dtype=torch.float64, device=self.device)
+        args = [tp, gp, nclass, stats.shape[0] if stats is not None else 0, sp, C.c_void_p(loss_target.data_ptr()),
+                int(ignore_index), C.c_void_p(acc.data_ptr()), C.c_void_p(part.data_ptr()), part.numel()]
+        return args, (target, g, loss_target, part)
+
+    def forward_loss(self, x, text, k, loss_target, acc, ignore_index=-1, text_image_stride=0, target=None, stats=None,
+                     nclass=0, group=None, mask=None, logits=None):
+        """Forward with the cross-entropy fused into the output kernel: adds {sum of per-pixel losses, counted pixels} of
+        the logits against loss_target int64 [B,H,W] (pixels equal to ignore_index skipped) to acc float64 [2]. With
+        target and stats, also the metric counters as forward_stats adds them; mask / logits are written when passed.
+        Enqueues on the current stream and does not synchronise."""
+        self._check_input(x)
+        x = x.contiguous()
+        b, _, h, w = x.shape
+        args, keep = self._loss_args(b, h, w, k, loss_target, acc, ignore_index, target, stats, nclass, group, mask,
+                                     logits)
+        mp = C.c_void_p(mask.data_ptr()) if mask is not None else None
+        lp = C.c_void_p(logits.data_ptr()) if logits is not None else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_forward_xent(self.handle, C.c_void_p(x.data_ptr()), b, h, w,
+                                                  C.c_void_p(text.data_ptr()), k, text_image_stride, *args, mp, lp,
+                                                  _stream()))
+        return acc
+
+    def query_loss(self, emb, sumsq, text, k, loss_target, acc, ignore_index=-1, text_image_stride=0, target=None,
+                   stats=None, nclass=0, group=None, mask=None, logits=None):
+        """forward_loss's label-dependent tail on a stored embedding pair: the same bits as forward_loss on the images
+        that produced it."""
+        b, h, w = check_embedding(emb, sumsq, self.device, self.out_c)
+        args, keep = self._loss_args(b, h, w, k, loss_target, acc, ignore_index, target, stats, nclass, group, mask,
+                                     logits)
+        mp = C.c_void_p(mask.data_ptr()) if mask is not None else None
+        lp = C.c_void_p(logits.data_ptr()) if logits is not None else None
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.lseg_query_xent(self.handle, C.c_void_p(emb.data_ptr()), C.c_void_p(sumsq.data_ptr()),
+                                                b, h, w, C.c_void_p(text.data_ptr()), k, text_image_stride, lp, mp,
+                                                *args, _stream()))
+        return acc
+
     def encode_image(self, x):
         """The image path of forward (trunk, decoder, head1) -> the pixel embedding pair (emb fp16 [B,H/2,W/2,out_c],
         sumsq fp32 [B,H/2,W/2,out_c/32]); layout in include/lseg_b200.h. Enqueues on the current stream."""

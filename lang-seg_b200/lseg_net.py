@@ -606,6 +606,36 @@ class LSegNet(_LSegBase):
             engine.forward_stats(x.float(), feats, text.shape[0], t, stats, metric.nclass)
 
 
+    @torch.no_grad()
+    def loss(self, x, target, labelset="", ignore_index=-1, metric=None):
+        """F.cross_entropy(self.forward(x, labelset), target, ignore_index=ignore_index) — the validation loss of
+        LSegmentationModule.validation_step — fused into the output kernel: a 0-d fp32 CUDA tensor, computed without
+        writing the logits and without synchronising. target int64 [B,H,W] (or [H,W] for B = 1). A target outside
+        [0, K) other than ignore_index makes the loss NaN and is recorded on the device (lseg_read_watchdog tag 79, which
+        FewShotMeter.compute_iou raises on) where torch would assert. With `metric` (a lseg_b200.metrics.SegmentationMetric), its counters are added in the
+        same kernel, exactly as update_metric adds them."""
+        from .metrics import _as_target, _mean_loss
+        self._check_eval()
+        if is_ragged(labelset):
+            raise ValueError("loss does not take per-image label sets: the class ids of the target would differ from "
+                             "image to image")
+        text = self._labelset_tokens(labelset)
+        x = self._image_path(x)
+        emb = x if isinstance(x, PixelEmbedding) else None
+        engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
+        feats = self._text_features(engine, text)
+        t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
+        acc = torch.zeros(2, dtype=torch.float64, device=x.device)
+        kw = dict(ignore_index=ignore_index)
+        if metric is not None:
+            kw.update(target=t, stats=metric._buffer(x.device), nclass=metric.nclass)
+        if emb is not None:
+            engine.query_loss(emb.emb, emb.sumsq, feats, text.shape[0], t, acc, **kw)
+        else:
+            engine.forward_loss(x.float(), feats, text.shape[0], t, acc, **kw)
+        return _mean_loss(acc)
+
+
 class LSegNetZS(_LSegBase):
     """Zero-shot variant (reference: lseg_net_zs.py:219-239; forward :177-214): one ['others', name]
     prompt pair per image, selected by class_info."""
@@ -697,6 +727,36 @@ class LSegNetZS(_LSegBase):
                          group=group)
         else:
             engine.forward_stats(x.float(), text, 2, t, meter.stats, 2, group=group, text_image_stride=2)
+
+
+    @torch.no_grad()
+    def loss(self, x, class_info, target, ignore_index=-1, meter=None, query_ignore_idx=None):
+        """criterion(self.forward(x, class_info), target) of the zero-shot validation step (CrossEntropyLoss with
+        ignore_index over the raw target), fused into the output kernel: a 0-d fp32 CUDA tensor. With `meter` (a
+        lseg_b200.metrics.FewShotMeter), the same kernel also adds the update_metric counters (the metric target gets
+        query_ignore_idx applied, the loss target does not) and the loss is appended to meter.loss_buf. A target outside
+        [0, 2) other than ignore_index (e.g. 255 with ignore_index=-1) gives NaN and a device record instead of torch's
+        assert."""
+        from .metrics import _as_target, _fewshot_target, _mean_loss
+        self._check_eval()
+        x = self._image_path(x)
+        emb = x if isinstance(x, PixelEmbedding) else None
+        engine = self._embedding_engine(emb) if emb is not None else self._engine_for(x.device)
+        text = self._image_text(engine, class_info, x.device)
+        t = _as_target(target, x.device, (x.shape[0], x.shape[2], x.shape[3]))
+        acc = torch.zeros(2, dtype=torch.float64, device=x.device)
+        kw = dict(ignore_index=ignore_index, text_image_stride=2)
+        if meter is not None:
+            kw.update(target=_fewshot_target(t, query_ignore_idx), stats=meter.stats, nclass=2,
+                      group=torch.as_tensor(class_info).to(x.device))
+        if emb is not None:
+            engine.query_loss(emb.emb, emb.sumsq, text, 2, t, acc, **kw)
+        else:
+            engine.forward_loss(x.float(), text, 2, t, acc, **kw)
+        loss = _mean_loss(acc)
+        if meter is not None:
+            meter.loss_buf.append(loss)
+        return loss
 
 
 class LSegRNNetZS(LSegNetZS):

@@ -33,6 +33,12 @@ would fail) is not counted; the kernel records it on the device and FewShotMeter
 (lseg_read_watchdog, tag 78). The record belongs to the device, not to one meter: it is raised by the next
 compute_iou() on that device.
 
+The validation loss (SegmentationLosses here, LSegNet.loss / LSegNetZS.loss fused into the output kernel) is
+CrossEntropyLoss(ignore_index) with mean reduction: per pixel (m + log s) - v_t in fp32 over the classes' logits
+(include/lseg_b200.h, section "cross-entropy"), summed in fp64 in a fixed order, so a call gives the same bits every time.
+A target outside [0, K) other than ignore_index, where torch's CUDA kernel asserts and ends the process's CUDA context,
+makes the loss NaN and is recorded on the device (tag 79); FewShotMeter.compute_iou() raises on that record.
+
 Differences from the reference classes: the counters are int64 (the reference's float32 AverageMeter buffers round above
 2^24 pixels per class) and are converted only when read; classify_prediction does not modify its arguments (the reference
 writes 255 into pred_mask and multiplies query_ignore_idx in place) and returns int64 counts; everything runs on CUDA only.
@@ -44,6 +50,7 @@ from . import ops
 
 
 SEGSTATS_TAG = 78  # lseg_read_watchdog tag of an image skipped for a row id outside [0, rows)
+XENT_TAG = 79  # lseg_read_watchdog tag of a loss target outside [0, K) that is not ignore_index
 
 
 def _raise_on_device_error(device):
@@ -53,6 +60,9 @@ def _raise_on_device_error(device):
     if wd[0] == SEGSTATS_TAG:
         raise RuntimeError(f"a metric update skipped image {wd[1]} of its batch: its row id {wd[2]} is outside [0, {wd[3]}) "
                            f"(class_info beyond the meter's nclass?); the counters miss that image")
+    if wd[0] == XENT_TAG:
+        raise RuntimeError(f"a loss call met target {wd[3]} at pixel {wd[2]} (y * W + x) of image {wd[1]} of its batch: "
+                           f"outside [0, K) and not ignore_index; that loss is NaN")
     if wd[0] != 0:
         raise RuntimeError(f"a kernel's barrier watchdog fired on {device} (tag {wd[0]}): results since the last check are "
                            f"not trustworthy")
@@ -98,6 +108,48 @@ def _accumulate(stats, nclass, output, target, group=None):
         raise ValueError(f"prediction must be scores [B,K,H,W] (float) or a class mask [B,H,W] (integer), got "
                          f"{output.dtype} {tuple(output.shape)}")
     return stats
+
+
+def _mean_loss(acc):
+    """0-d fp32 mean of a loss accumulator {sum, count} (float64 [2]); NaN when every pixel was ignored, as in torch."""
+    return (acc[0] / acc[1]).float()
+
+
+class SegmentationLosses:
+    """PyTorch-Encoding's SegmentationLosses (the criterion of LSegmentationModule.get_criterion) for what LSeg uses
+    of it: with se_loss = aux = False and no class weight it is CrossEntropyLoss(ignore_index) with mean reduction,
+    computed here by one device kernel over the fp32 scores [B,K,H,W] without torch's log_softmax intermediate. The loss
+    terms LSeg never produces inputs for (se_loss, aux, class weights) raise NotImplementedError. A target outside
+    [0, K) other than ignore_index gives NaN and a device record (lseg_read_watchdog tag 79) where torch would assert."""
+
+    def __init__(self, se_loss=False, se_weight=0.2, nclass=-1, aux=False, aux_weight=0.4, weight=None,
+                 ignore_index=-1):
+        if se_loss:
+            raise NotImplementedError("se_loss: LSeg's net returns no SE-loss prediction")
+        if aux:
+            raise NotImplementedError("aux: LSeg's net returns no auxiliary output")
+        if weight is not None:
+            raise NotImplementedError("class weights are not supported")
+        self.se_loss, self.aux = se_loss, aux
+        self.nclass = nclass
+        self.se_weight, self.aux_weight = se_weight, aux_weight
+        self.ignore_index = int(ignore_index)
+
+    def __call__(self, *inputs):
+        if len(inputs) != 2:
+            raise ValueError(f"SegmentationLosses takes (scores, target), got {len(inputs)} arguments")
+        scores, target = inputs
+        if not scores.is_cuda:
+            raise ValueError("lseg_b200.metrics runs on CUDA only: the scores must be a CUDA tensor")
+        if scores.dim() != 4 or not scores.is_floating_point():
+            raise ValueError(f"scores must be float [B,K,H,W], got {scores.dtype} {tuple(scores.shape)}")
+        scores = scores.float().contiguous()
+        t = _as_target(target, scores.device, (scores.shape[0],) + tuple(scores.shape[2:]))
+        acc = torch.zeros(2, dtype=torch.float64, device=scores.device)
+        ops.xent_scores(scores, t, acc, self.ignore_index)
+        return _mean_loss(acc)
+
+    forward = __call__
 
 
 def _batch_row(output, target, nclass):
@@ -210,6 +262,7 @@ class FewShotMeter:
             raise ValueError("lseg_b200.metrics runs on CUDA only")
         self.class_ids_interest = torch.as_tensor(class_ids, dtype=torch.int64).to(device)
         self.stats = torch.zeros((self.nclass, _row_len(2)), dtype=torch.int64, device=device)
+        self.loss_buf = []  # one loss per update (LSegNetZS.loss with meter= appends its own)
 
     @property
     def intersection_buf(self):
@@ -220,10 +273,9 @@ class FewShotMeter:
         return (self.stats[:, 2:4] + self.stats[:, 4:6] - self.stats[:, 0:2]).t()
 
     def update(self, inter_b, union_b, class_id, loss=None):
-        """Adds [2, B] counts to the rows class_id [B] (AverageMeter.update's index_add_). `loss` exists for call
-        compatibility with test_lseg_zs.py, which passes None; a loss is not kept."""
-        if loss is not None:
-            raise NotImplementedError("FewShotMeter keeps no loss buffer")
+        """Adds [2, B] counts to the rows class_id [B] (AverageMeter.update's index_add_) and appends `loss` to loss_buf
+        (torch.tensor(0.0) for None, as AverageMeter does)."""
+        self.loss_buf.append(torch.tensor(0.0) if loss is None else loss)
         cid = torch.as_tensor(class_id).to(device=self.stats.device, dtype=torch.int64).reshape(-1)
         inter = inter_b.to(device=self.stats.device, dtype=torch.int64).t()
         union = union_b.to(device=self.stats.device, dtype=torch.int64).t()
@@ -246,3 +298,4 @@ class FewShotMeter:
 
     def reset(self):
         self.stats.zero_()
+        self.loss_buf = []

@@ -398,6 +398,25 @@ def seg_stats_mask(pred, target, stats, nclass, group=None):
     return stats
 
 
+def xent_partials(B, H, W, fused):
+    """(sum, count) fp64 pairs of partials a loss call needs (include/lseg_b200.h): one per block of the loss kernel."""
+    return B * ((H + 7) // 8) if fused else B * ((H * W + 1023) // 1024)
+
+
+def xent_scores(scores, target, acc, ignore_index=-1):
+    """Adds {sum of per-pixel cross-entropies, counted pixels} of fp32 scores [B,K,H,W] against int64 target [B,H,W]
+    (pixels equal to ignore_index skipped) to acc float64 [2]. Enqueues on the current stream."""
+    B, K, H, W = scores.shape
+    if tuple(target.shape) != (B, H, W):
+        raise ValueError(f"target must be [B,H,W] = {(B, H, W)}, got {tuple(target.shape)}")
+    if acc.dtype != torch.float64 or acc.numel() != 2 or not acc.is_contiguous():
+        raise ValueError("acc must be a contiguous float64 tensor of 2 elements")
+    part = torch.empty((xent_partials(B, H, W, False), 2), dtype=torch.float64, device=scores.device)
+    check(load().lseg_xent_scores(_ptr(scores, torch.float32), _ptr(target, torch.int64), int(ignore_index), B, K, H, W,
+                                  _ptr(acc, torch.float64), _ptr(part), part.numel(), _stream()))
+    return acc
+
+
 def text_embed(tokens, tok_emb, pos_emb, out=None):
     K, L = tokens.shape
     Wd = tok_emb.shape[1]
